@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — event tokens/sec of the Mapperatorinator inference hot path on B200 (contract: see README "Measurement").
+"""bench.py — event tokens/sec of the Mapperatorinator inference hot path on H100 (see README "Measurement").
 
 Workload (BASELINE.json configs[1] + configs[2], SURVEY §8d rows 2a + 3): osuT5 v29 dimensions (whisper-small, 213 M params,
 fp32, seeded random weights), one 180 s synthetic song as 44.1 kHz 16-bit stereo PCM -> GPU ingest (resample to 16 kHz, mono, peak-normalise) -> 211 sequential windows (stride 13 094 samples), greedy decode,
@@ -21,6 +21,9 @@ A "step" = one full song (decode + position refinement).
   --impl reference : the CPU oracle port of the reference path (same call pattern) on the host cores, bounded sample.
 Multi-GPU (torchrun): one song per rank per step (weak scaling; rank r decodes song `--song-seed + r`), NCCL gather of the
 token streams inside the timed region.
+--dump-outputs DIR : after the timed steps, rank 0 writes what the resident arm's last timed step returned — the generated token ids of
+          every window (tokens.npy, float64 [songs, windows, tokens], -1 padded) and the refined DiT positions (positions.npy, float32
+          [songs, 2, points]) — so that two builds can be compared output for output (the inputs are seeded: identical run to run).
 """
 from __future__ import annotations
 
@@ -126,7 +129,7 @@ def dit_chunks(T: int = DIT_POINTS):
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region."""
     Q = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, index: int):
@@ -166,7 +169,7 @@ def workload_config(n_windows: int, dit: bool, songs_per_gpu: int = 1) -> dict:
                        + (" + osu_diffusion DiT-B 100-step position refinement (configs[2], SURVEY 8d 3)" if dit else ""),
            "windows": n_windows, "new_tokens_per_window": NEW_TOKENS, "decode": "greedy, min_new_tokens=64", "batch": songs_per_gpu,
            "weights": "seeded random init, whisper-small dims (213M) + DiT-B (131M), fp32", "songs_per_gpu_per_step": songs_per_gpu,
-           "l2": "inputs larger than L2: each token streams the 464 MB fp32 decoder (L2 = 126 MB)"}
+           "l2": "inputs larger than L2: each token streams the 464 MB fp32 decoder (H100 L2 = 50 MB)"}
     if dit:
         cfg["dit"] = {"points": DIT_POINTS, "chunks": dit_chunks(), "steps": DIT_STEPS, "cfg_pair": True, "band": 128}
     return cfg
@@ -275,6 +278,19 @@ def first_stream_divergence(a, b):
     return None if len(a) == len(b) else {"window": min(len(a), len(b)), "token": 0, "resident": None, "e2e": None}
 
 
+def dump_outputs(out_dir: str, streams, pos) -> None:
+    """The last timed step's results as a caller receives them: token ids per (song, window), -1 padded, and DiT positions per song."""
+    os.makedirs(out_dir, exist_ok=True)
+    n_tok = max((len(w) for st in streams for w in st), default=0)
+    ids = np.full((len(streams), max(len(st) for st in streams), n_tok), -1.0, dtype=np.float64)
+    for k, st in enumerate(streams):
+        for i, w in enumerate(st):
+            ids[k, i, :len(w)] = w
+    np.save(os.path.join(out_dir, "tokens.npy"), ids)
+    if pos is not None:
+        np.save(os.path.join(out_dir, "positions.npy"), np.stack([p.float().cpu().numpy() for p in pos]).astype(np.float32))
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -292,10 +308,11 @@ def main() -> None:
                     help="N=1: teacher-forced oracle check of the GPU's greedy ids over the whole song / every 8th window / not at all")
     ap.add_argument("--pdl", type=int, default=int(os.environ.get("MB200_PDL", "0")))
     ap.add_argument("--windows", type=int, default=0, help="debug: truncate the song to this many windows")
-    ap.add_argument("--tc", type=int, default=int(os.environ.get("MB200_TC", "1")), help="1 = tcgen05 3xTF32 GEMMs where eligible, 0 = fp32 SIMT GEMM everywhere")
+    ap.add_argument("--tc", type=int, default=int(os.environ.get("MB200_TC", "1")), help="1 = wgmma 3xTF32 GEMMs where eligible, 0 = fp32 SIMT GEMM everywhere")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write the last timed step's token ids and DiT positions as DIR/*.npy")
     ap.add_argument("--mega", type=int, default=2, help="2 = dataflow token-loop megakernel (default), 1 = grid-barrier megakernel, 0 = CUDA-graph replay per token")
     ap.add_argument("--cpu-threads", type=int, default=int(os.environ.get("MB200_CPU_THREADS", "0")),
-                    help="torch threads of the CPU arm (0 = min(cores, 16): measured best on the GPU box; 32+ threads slow a batch-1 decoder down)")
+                    help="torch threads of the CPU arm (0 = min(cores, 16): 32+ threads slow a batch-1 decoder down)")
     args = ap.parse_args()
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
     if args.impl == "reference":
@@ -437,6 +454,8 @@ def main() -> None:
     n_ev = max(1, len(step_resident.events))
     stage_ms = {k: v / n_ev for k, v in stage_ms.items()}
     mega_resident, ms_resident = timed.mega, ms
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, streams, pos)
     e2e_steps = max(1, args.steps // 2)
     ms_e2e, toks_e2e, _, streams2, pos2 = timed(step_e2e, e2e_steps, 1)
     # the two arms must emit the same tokens (and positions): reported, not asserted, so every rank always prints / exits cleanly
@@ -460,19 +479,8 @@ def main() -> None:
     w_bytes = 4 * (L * (3 * d * d + 2 * d * d + d * d + 2 * d * f) + V * d)                  # decoder weights streamed once per token
     ctx = 50 + NEW_TOKENS // 2
     kv_bytes = 4 * L * 2 * (cfg.max_source_positions + ctx) * d                               # cross + self K/V read per token
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "MEASURED_PEAKS.json hbm_gbs (burst copy)" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
-    traffic, traffic_src = None, None
-    try:      # per-launch DRAM bytes of the token-loop kernel from the committed `ncu --set full` capture of this round
-        tr = json.load(open(os.path.join(ROOT, "profiles", "megakernel_traffic.json")))
-        traffic, traffic_src = tr["dram_bytes_per_launch"], tr["source"]
-    except Exception:
-        pass
+    peak = 3350.0
+    peak_src = "H100 SXM data sheet HBM3 bandwidth (not a measured peak)"
     mega = mega_resident
     if args.mega and mega[0] > 0:
         # persistent token-loop kernel: one launch per window decodes NEW_TOKENS-1 tokens; events recorded around every launch
@@ -482,9 +490,7 @@ def main() -> None:
         achieved = bytes_per_launch / (us_per_launch * 1e-6) / 1e9
         roofline = {"bound": "hbm", "kernel": ("decode_megakernel_ll<1> (dataflow megakernel" if args.mega >= 2 else "decode_megakernel<1> (grid-barrier megakernel")
                               + ": persistent cooperative kernel, all layers of all tokens of one generate() call)",
-                    "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                    "traffic": traffic if traffic and abs(tok_per_launch - 63.0) < 1e-6 else None, "traffic_source": traffic_src,
-                    "peak_source": peak_src, "bytes_per_launch": bytes_per_launch, "us_per_launch": us_per_launch, "tokens_per_launch": tok_per_launch,
+                    "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src, "bytes_per_launch": bytes_per_launch, "us_per_launch": us_per_launch, "tokens_per_launch": tok_per_launch,
                     "us_per_token": us_per_launch / tok_per_launch, "bytes_per_token": w_bytes + kv_bytes,
                     "share_of_step": mega[1] / (ms_resident), "token_floor_us": (w_bytes + kv_bytes) / (peak * 1e3)}
     else:
@@ -494,8 +500,7 @@ def main() -> None:
         gemv_us = float(out_us[0])
         achieved = (w_bytes / n_gemv) / (gemv_us / n_gemv * 1e-6) / 1e9 if gemv_us > 0 else None
         roofline = {"bound": "hbm", "kernel": f"gemv_kernel<1> ({n_gemv} launches per token, CUDA-graph path; eager event timing includes launch gaps)",
-                    "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak if achieved else None, "traffic": None,
-                    "peak_source": peak_src, "bytes_per_launch": w_bytes / n_gemv, "us_per_launch": gemv_us / n_gemv,
+                    "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak if achieved else None, "peak_source": peak_src, "bytes_per_launch": w_bytes / n_gemv, "us_per_launch": gemv_us / n_gemv,
                     "per_token_us": {"gemv": gemv_us, "attention": float(out_us[1]), "sample": float(out_us[2])},
                     "token_floor_us": (w_bytes + kv_bytes) / (peak * 1e3)}
 
@@ -570,6 +575,6 @@ if __name__ == "__main__":
     except SystemExit:
         raise
     except BaseException:
-        # a rank that dies must say who it was and why, on stdout (torchrun interleaves stderr and the driver keeps stdout)
+        # a rank that dies must say who it was and why, on stdout (torchrun interleaves stderr; stdout carries the JSON lines)
         print(json.dumps({"rank": int(os.environ.get("RANK", 0)), "error": traceback.format_exc()}), flush=True)
         sys.exit(1)

@@ -1,4 +1,4 @@
-/* mapperatorinator_b200 — C ABI of the Blackwell-native engine for the Mapperatorinator inference hot path.
+/* mapperatorinator_b200 — C ABI of the H100-native (sm_90a) engine for the Mapperatorinator inference hot path.
  *
  * The reference (OliBomby/Mapperatorinator) has no FFI layer: its boundary is a Python object protocol (SURVEY §8b).
  * Each entry point below names the reference call it replaces.  All pointers are plain device or host pointers owned by
@@ -199,7 +199,7 @@ int mb200_model_mega_stats(mb200_model* m, double* out, int32_t reset);
 int mb200_op_gemm(const float* A, int64_t lda, const float* W, int64_t ldw, float* C, int64_t ldc, const float* bias, int32_t act,
                   float alpha, const float* residual, int64_t ldr, const float* gate, int64_t gate_ld, int32_t gate_rpb, int32_t M,
                   int32_t N, int32_t K, void* cuda_stream);
-/* the tcgen05 3xTF32 GEMM on its own (registers W's lo mirror, runs, synchronises, checks the pipeline error flag) */
+/* the wgmma 3xTF32 GEMM on its own (registers W's lo mirror, runs, synchronises, checks the pipeline error flag) */
 int mb200_op_gemm_tc(const float* A, int64_t lda, const float* W, int64_t ldw, float* C, int64_t ldc, const float* bias, int32_t act,
                      float alpha, const float* residual, int64_t ldr, int32_t M, int32_t N, int32_t K, void* cuda_stream);
 /* 0 = route every GEMM through the fp32 SIMT kernel (A/B comparisons), 1 = tensor cores where eligible (default) */
@@ -209,7 +209,7 @@ int mb200_op_layernorm(const float* x, float* y, const float* w, const float* b,
 int mb200_op_attention(const float* q, const float* k, const float* v, float* o, int32_t B, int32_t H, int32_t Tq, int32_t Tk,
                        float scale, int32_t mask_mode, int32_t q_pos0, const uint8_t* key_valid, int32_t band,
                        const uint8_t* dense_mask, void* cuda_stream);
-/* Tuning / tests: tensor-core (tcgen05, 3xTF32) flash attention on or off, and the minimum number of queries for which it is used
+/* Tuning / tests: tensor-core (wgmma, 3xTF32) flash attention on or off, and the minimum number of queries for which it is used
    (attention_tc.cu; replaces the SIMT kernel for the encoder self-attention of HF modeling_whisper.py:286-358 and the DiT band of
    osu_diffusion/utils/models.py:145-151). */
 int mb200_set_attention_tc(int32_t enabled, int32_t min_queries);

@@ -67,7 +67,7 @@ def load() -> C.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            f"{LIB_PATH} is not built. mapperatorinator_b200 has no CPU fallback: build the sm_100a engine with "
+            f"{LIB_PATH} is not built. mapperatorinator_b200 has no CPU fallback: build the sm_90a engine with "
             "`python -c 'import __graft_entry__ as g; g.build()'` (or mapperatorinator_b200/csrc/build.sh).")
     lib = C.CDLL(LIB_PATH)
     lib.mb200_last_error.restype = C.c_char_p

@@ -1,17 +1,18 @@
 // Tensor-core flash attention (head_dim 64) for the dense phases: Whisper encoder self-attention (T = 512, HF modeling_whisper.py:286-358),
 // the DiT blocks' +-128 band (osu_diffusion/utils/models.py:145-151) and causal / key-padded self-attention.  fp32 in, fp32 out, both
-// contractions on tcgen05.mma kind::tf32 with the 3xTF32 split of gemm_tc.cu (x = hi + lo, hi.hi + hi.lo + lo.hi), accumulators in TMEM.
+// contractions on Hopper wgmma (kind tf32) with the 3xTF32 split of gemm_tc.cu (x = hi + lo, hi.hi + hi.lo + lo.hi), fp32 accumulators
+// in registers.
 //
 //   attn_prep_kernel   one pass over q | k | v (token-major, the projection GEMM's layout): scale + tf32 hi / lo split, written head-major
 //                      as Q [2][B*H][Tq_pad][64], K [2][B*H][Tk_pad][64] and V TRANSPOSED VT [2][B*H][64][Tk_pad] (so that V is a K-major
-//                      B operand of the second contraction), zero padded to whole tiles.
-//   attention_tc_kernel  one CTA = 128 queries of one (batch, head), 64-key tiles, 192 threads:
-//       warp 0 / lane 0 : TMA producer — Q once (4 x [128 x 32 floats]), then per KV tile 4 K tiles + 4 VT tiles (2-stage ring)
-//       warp 1 / lane 0 : MMA issuer   — S = Q K^T (24 x tcgen05.mma 128x64x8, SS) into one of two 64-column TMEM buffers, issued one tile
-//                         AHEAD; O_t = P V (24 x tcgen05.mma, TS: P is read from TMEM) into a third buffer
-//       warps 2..5      : one thread per query row (its TMEM lane): tcgen05.ld S -> mask -> online softmax in registers -> P hi / lo back to
-//                         TMEM (tcgen05.st) -> after the PV MMA: O <- O * alpha + O_t in registers -> normalise -> 256 contiguous bytes per row
-//   Row max, row sum and the running output never leave the thread that owns the row: no shuffles, no shared-memory softmax.
+//                      B operand of the second contraction), zero padded to whole tiles.  Inside every group of 8 keys VT holds the keys
+//                      in the order 0 2 4 6 1 3 5 7: that is the order in which a thread's score accumulators (keys 2t, 2t+1) sit in the
+//                      A-operand fragment of the P.V MMA (columns t, t+4), so P goes from the score registers into the MMA unshuffled.
+//   attention_tc_kernel  one CTA = 128 queries of one (batch, head), 64-key tiles, 384 threads (3 warpgroups):
+//       warpgroup 0, thread 0 : TMA producer — Q once (4 x [128 x 32 floats]), then per KV tile 4 K tiles + 4 VT tiles (2-stage ring)
+//       warpgroups 1, 2       : 64 query rows each: S = Q K^T (24 x wgmma m64n64k8, both operands in shared memory) -> mask -> online
+//                               softmax in registers (a row lives in the 4 threads of a quad) -> O = O * alpha + P V (24 x wgmma
+//                               m64n64k8, P hi / lo from registers) -> normalise -> store.
 // Every wait is bounded (error flag + fall through), like gemm_tc.cu.  Dense boolean masks and K/V gathered through kv_slot stay on the
 // fp32 SIMT kernel (attention.cu).
 #include <cuda.h>
@@ -22,27 +23,21 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace mb200 {
 
 namespace {
 
-constexpr int FA_BM = 128, FA_BN = 64, FA_HD = 64, FA_THREADS = 320, FA_STAGES = 2;      // TMA warp + MMA warp + 8 softmax warps
+constexpr int FA_BM = 128, FA_BN = 64, FA_HD = 64, FA_THREADS = 384, FA_CONSUMERS = 256, FA_STAGES = 2;
 constexpr int FA_Q_TILE = FA_BM * 32 * 4;                 // 16 KB: 128 rows x 32 floats
 constexpr int FA_Q_BYTES = 4 * FA_Q_TILE;                 // hi d0-31 | hi d32-63 | lo d0-31 | lo d32-63
 constexpr int FA_KV_TILE = FA_BN * 32 * 4;                // 8 KB: 64 rows x 32 floats
 constexpr int FA_STAGE_BYTES = 8 * FA_KV_TILE;            // K: hi d0, hi d1, lo d0, lo d1 | VT: hi k0, hi k1, lo k0, lo k1
-constexpr unsigned FA_TM_S0 = 0, FA_TM_S1 = 64, FA_TM_PHI = 128, FA_TM_PLO = 192, FA_TM_OT = 256, FA_TM_COLS = 512;
 
 struct FaBarriers {
     unsigned long long q_full;
     unsigned long long kv_full[FA_STAGES], kv_empty[FA_STAGES];
-    unsigned long long s_full[2];
-    unsigned long long p_full;        // 256 softmax threads arrive
-    unsigned long long o_full;
-    unsigned int tmem_base;
-    int pad;
-    float xchg[2][2][FA_BM];          // [tile parity][column half][row]: row maxima of the two threads that share a query row
 };
 
 __device__ __forceinline__ unsigned fa_s32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -57,53 +52,15 @@ __device__ __forceinline__ bool fa_wait(unsigned long long* bar, unsigned parity
     atomicExch(err, 5);
     return false;
 }
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (see gemm_tc.cu)
-__device__ __forceinline__ unsigned long long fa_desc(unsigned smem_addr) {
-    unsigned long long d = 0;
-    d |= (unsigned long long)((smem_addr >> 4) & 0x3FFF);
-    d |= (unsigned long long)1 << 16;
-    d |= (unsigned long long)(1024 >> 4) << 32;
-    d |= (unsigned long long)1 << 46;
-    d |= (unsigned long long)2 << 61;
-    return d;
-}
-__device__ __forceinline__ void fa_mma_ss(unsigned tmem_d, unsigned long long da, unsigned long long db, unsigned idesc, unsigned acc) {
-    asm volatile("{ .reg .pred p; setp.ne.b32 p, %4, 0; tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p; }"
-                 ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void fa_mma_ts(unsigned tmem_d, unsigned tmem_a, unsigned long long db, unsigned idesc, unsigned acc) {
-    asm volatile("{ .reg .pred p; setp.ne.b32 p, %4, 0; tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p; }"
-                 ::"r"(tmem_d), "r"(tmem_a), "l"(db), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void fa_commit(unsigned long long* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"l"(__cvta_generic_to_shared(bar)) : "memory");
-}
-__device__ __forceinline__ void fa_tmem_ld32(unsigned (&v)[32], unsigned taddr) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, "
-        "%20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void fa_tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void fa_tmem_st32(unsigned taddr, const unsigned (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, "
-        "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-          "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]),
-          "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]),
-          "r"(v[30]), "r"(v[31])
-        : "memory");
-}
 __device__ __forceinline__ float fa_rn_tf32(float x) {
     unsigned u;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
     return __uint_as_float(u);
+}
+__device__ __forceinline__ float fa_ex2(float x) {
+    float y;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
 }
 
 struct FaParams {
@@ -121,7 +78,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
     unsigned char* q_s = smem;
     unsigned char* kv_s = smem + FA_Q_BYTES;
     FaBarriers* bars = reinterpret_cast<FaBarriers*>(smem + FA_Q_BYTES + FA_STAGES * FA_STAGE_BYTES);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x;
     const int q0 = blockIdx.x * FA_BM, bh = blockIdx.y, b = bh / p.H, h = bh - b * p.H;
 
     // KV tile range the mask allows for this query tile
@@ -140,25 +97,15 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
         asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(fa_s32(&bars->q_full)));
         for (int s = 0; s < FA_STAGES; ++s) {
             asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(fa_s32(&bars->kv_full[s])));
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(fa_s32(&bars->kv_empty[s])));
+            asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(fa_s32(&bars->kv_empty[s])), "r"(FA_CONSUMERS));
         }
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(fa_s32(&bars->s_full[0])));
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(fa_s32(&bars->s_full[1])));
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 256;" ::"r"(fa_s32(&bars->p_full)));
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(fa_s32(&bars->o_full)));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(fa_s32(&bars->tmem_base)), "r"(FA_TM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const unsigned tmem = bars->tmem_base;
 
-    if (warp == 0) {
-        if (lane == 0 && ntiles > 0) {
+    if (tid < 128) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (tid == 0 && ntiles > 0) {
             // Q: rows bh * Tq_pad + q0 .. +127, halves d0-31 / d32-63, hi (plane 0) then lo (plane 1)
             const unsigned qb = fa_s32(&bars->q_full);
             asm volatile("{ .reg .b64 t; mbarrier.arrive.expect_tx.shared::cta.b64 t, [%0], %1; }" ::"r"(qb), "r"(FA_Q_BYTES) : "memory");
@@ -183,147 +130,143 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
                                  ::"r"(fa_s32(st + (4 + t) * FA_KV_TILE)), "l"(&map_vt), "r"(k0 + (t & 1) * 32), "r"(bh * FA_HD), "r"(t >> 1), "r"(fb) : "memory");
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0 && ntiles > 0) {
-            // instruction descriptor: D fp32, A / B tf32, both K-major, N = 64, M = 128
-            const unsigned idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((unsigned)(FA_BN >> 3) << 17) | ((unsigned)(FA_BM >> 4) << 24);
-            bool ok = fa_wait(&bars->q_full, 0, err);
-            const unsigned qa = fa_s32(q_s);
-            auto issue_s = [&](int i) {          // S_i = Q K_i^T into TMEM buffer i & 1
-                const int s = i % FA_STAGES;
-                ok = ok && fa_wait(&bars->kv_full[s], (i / FA_STAGES) & 1, err);
-                if (!ok) return;
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const unsigned kb = fa_s32(kv_s + s * FA_STAGE_BYTES);
-                const unsigned acc = tmem + ((i & 1) ? FA_TM_S1 : FA_TM_S0);
+        return;
+    }
+
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // ---- consumer warpgroup g: query rows 64 g .. +63 of the tile.  Thread (warp w, lane = 4 gid + tig) holds rows r = 16 w + gid and
+    //      r + 8, score / output columns 8 j + 2 tig + {0, 1} (j = 0..7); a row's max and sum are reduced over its quad.
+    //      Scores arrive in the log2 domain (scale * log2 e folded into Q by the prep pass): p = ex2(s - m) is one MUFU instruction.
+    const int ct = tid - 128, g = ct >> 7, w = (ct >> 5) & 3, lane = ct & 31, gid = lane >> 2, tig = lane & 3;
+    const int qr[2] = {q0 + g * 64 + w * 16 + gid, q0 + g * 64 + w * 16 + gid + 8};
+    const unsigned qa = fa_s32(q_s) + (unsigned)g * (64 * 128);           // this warpgroup's 64 Q rows inside each Q tile
+    const unsigned char* kvalid = p.key_valid ? p.key_valid + (long long)b * p.key_valid_ld : nullptr;
+    // keys a row may see form one interval [k_lo, k_hi) (none / causal / band); key padding is applied on top when present
+    int k_lo[2], k_hi[2];
 #pragma unroll
-                for (int ks = 0; ks < 8; ++ks) {         // 8 k-steps of 8 dims: tile ks / 4, 32-byte sub-step ks % 4
-                    const unsigned qo = (ks >> 2) * FA_Q_TILE + (ks & 3) * 32, ko = (ks >> 2) * FA_KV_TILE + (ks & 3) * 32;
-                    const unsigned long long q_hi = fa_desc(qa + qo), q_lo = fa_desc(qa + 2 * FA_Q_TILE + qo);
-                    const unsigned long long k_hi = fa_desc(kb + ko), k_lo = fa_desc(kb + 2 * FA_KV_TILE + ko);
-                    fa_mma_ss(acc, q_hi, k_hi, idesc, ks > 0 ? 1u : 0u);
-                    fa_mma_ss(acc, q_hi, k_lo, idesc, 1u);
-                    fa_mma_ss(acc, q_lo, k_hi, idesc, 1u);
-                }
-                fa_commit(&bars->s_full[i & 1]);
-            };
-            issue_s(0);
-            for (int i = 0; i < ntiles && ok; ++i) {
-                if (i + 1 < ntiles) issue_s(i + 1);      // the next tile's scores are computed while the softmax warps work on this one
-                ok = ok && fa_wait(&bars->p_full, i & 1, err);
-                if (!ok) break;
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const int s = i % FA_STAGES;
-                const unsigned vb = fa_s32(kv_s + s * FA_STAGE_BYTES + 4 * FA_KV_TILE);
+    for (int e = 0; e < 2; ++e) {
+        const int q = qr[e];
+        k_lo[e] = 0; k_hi[e] = p.Tk;
+        if (p.mask_mode == MASK_CAUSAL) k_hi[e] = min(k_hi[e], p.q_pos0 + q + 1);
+        else if (p.mask_mode == MASK_BAND) { k_lo[e] = max(k_lo[e], q - p.band + 1); k_hi[e] = min(k_hi[e], q + p.band + 1); }
+        if (q >= p.Tq) k_hi[e] = k_lo[e];
+    }
+    float o[32];
 #pragma unroll
-                for (int ks = 0; ks < 8; ++ks) {         // 8 k-steps of 8 keys: P columns ks * 8 .., V^T tile ks / 4
-                    const unsigned vo = (ks >> 2) * FA_KV_TILE + (ks & 3) * 32;
-                    const unsigned long long v_hi = fa_desc(vb + vo), v_lo = fa_desc(vb + 2 * FA_KV_TILE + vo);
-                    const unsigned p_hi = tmem + FA_TM_PHI + ks * 8, p_lo = tmem + FA_TM_PLO + ks * 8;
-                    fa_mma_ts(tmem + FA_TM_OT, p_hi, v_hi, idesc, ks > 0 ? 1u : 0u);
-                    fa_mma_ts(tmem + FA_TM_OT, p_hi, v_lo, idesc, 1u);
-                    fa_mma_ts(tmem + FA_TM_OT, p_lo, v_hi, idesc, 1u);
-                }
-                fa_commit(&bars->kv_empty[s]);           // K / V of this stage are free once these MMAs have read them
-                fa_commit(&bars->o_full);
-            }
+    for (int j = 0; j < 32; ++j) o[j] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    bool ok = ntiles == 0 || fa_wait(&bars->q_full, 0, err);
+#pragma unroll 1
+    for (int i = 0; i < ntiles && ok; ++i) {
+        const int s = i % FA_STAGES;
+        ok = fa_wait(&bars->kv_full[s], (i / FA_STAGES) & 1, err);
+        if (!ok) break;
+        const unsigned kb = fa_s32(kv_s + s * FA_STAGE_BYTES), vb = kb + 4 * FA_KV_TILE;
+        float sc[32];
+#pragma unroll
+        for (int j = 0; j < 32; ++j) sc[j] = 0.f;
+        gmma_fence_regs(sc);
+        gmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks) {         // 8 k-steps of 8 dims: tile ks / 4, 32-byte sub-step ks % 4
+            const unsigned qo = (ks >> 2) * FA_Q_TILE + (ks & 3) * 32, ko = (ks >> 2) * FA_KV_TILE + (ks & 3) * 32;
+            const unsigned long long q_hi = gmma_desc(qa + qo), q_lo = gmma_desc(qa + 2 * FA_Q_TILE + qo);
+            const unsigned long long k_hi = gmma_desc(kb + ko), k_lo = gmma_desc(kb + 2 * FA_KV_TILE + ko);
+            gmma_m64n64k8_ss(sc, q_hi, k_hi, ks > 0 ? 1u : 0u);
+            gmma_m64n64k8_ss(sc, q_hi, k_lo, 1u);
+            gmma_m64n64k8_ss(sc, q_lo, k_hi, 1u);
         }
-    } else {
-        // ---- softmax / output warps: TWO threads per query row (warps w and w + 4 share a TMEM lane group), 32 score / output columns each.
-        //      One warp per scheduler left every dependent instruction exposed (ncu: 20 k cycles per 64-key tile, tensor pipe 9 % active);
-        //      two warps per scheduler and half the columns per thread cut the per-tile chain four-fold.  Scores arrive in the log2 domain
-        //      (scale * log2 e folded into Q by the prep pass): p = ex2(s - m) is one MUFU instruction.
-        const int lg = warp & 3;                          // TMEM lane group this warp may access
-        const int half = (warp - 2) >> 2;                 // column half of this thread
-        const int row = lg * 32 + lane, q = q0 + row;
-        const unsigned lane_addr = (unsigned)(lg * 32) << 16;
-        const unsigned col0 = (unsigned)(half * 32);
-        float o[32];
+        gmma_commit();
+        gmma_wait<0>();
+        gmma_fence_regs(sc);
+
+        const int k0 = (kt_begin + i) * FA_BN;
+        float alpha[2];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) o[j] = 0.f;
-        float m_run = -INFINITY, l_run = 0.f;
-        bool ok = true;
-        const unsigned char* kvalid = p.key_valid ? p.key_valid + (long long)b * p.key_valid_ld : nullptr;
-        // keys this row may see form one interval [k_lo, k_hi) (none / causal / band); key padding is applied on top when present
-        int k_lo = 0, k_hi = p.Tk;
-        if (p.mask_mode == MASK_CAUSAL) k_hi = min(k_hi, p.q_pos0 + q + 1);
-        else if (p.mask_mode == MASK_BAND) { k_lo = max(k_lo, q - p.band + 1); k_hi = min(k_hi, q + p.band + 1); }
-        if (q >= p.Tq) k_hi = k_lo;
-        for (int i = 0; i < ntiles && ok; ++i) {
-            const int k0 = (kt_begin + i) * FA_BN + (int)col0;       // key of this thread's first column
-            ok = fa_wait(&bars->s_full[i & 1], (i >> 1) & 1, err);
-            if (!ok) break;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            unsigned sv[32];
-            fa_tmem_ld32(sv, tmem + lane_addr + ((i & 1) ? FA_TM_S1 : FA_TM_S0) + col0);
-            fa_tmem_ld_wait();
-            const int c_lo = k_lo - k0, c_hi = k_hi - k0;             // allowed columns of this thread: [c_lo, c_hi)
+        for (int e = 0; e < 2; ++e) {            // row e: accumulators 4 j + 2 e + {0, 1}
+            const int c_lo = k_lo[e] - k0, c_hi = k_hi[e] - k0;
             float mx = -INFINITY;
-            if (__all_sync(0xffffffffu, c_lo <= 0 && c_hi >= 32 && kvalid == nullptr)) {
+            if (c_lo <= 0 && c_hi >= FA_BN && kvalid == nullptr) {
 #pragma unroll
-                for (int c = 0; c < 32; ++c) mx = fmaxf(mx, __uint_as_float(sv[c]));
+                for (int j = 0; j < 8; ++j) mx = fmaxf(mx, fmaxf(sc[4 * j + 2 * e], sc[4 * j + 2 * e + 1]));
             } else {
 #pragma unroll
-                for (int c = 0; c < 32; ++c) {
-                    bool allowed = c >= c_lo && c < c_hi;
-                    if (kvalid) allowed = allowed && kvalid[min(k0 + c, p.Tk - 1)] != 0;
-                    const float sc = allowed ? __uint_as_float(sv[c]) : -INFINITY;
-                    sv[c] = __float_as_uint(sc);
-                    mx = fmaxf(mx, sc);
+                for (int j = 0; j < 8; ++j) {
+#pragma unroll
+                    for (int u = 0; u < 2; ++u) {
+                        const int c = 8 * j + 2 * tig + u;
+                        bool allowed = c >= c_lo && c < c_hi;
+                        if (kvalid) allowed = allowed && kvalid[min(k0 + c, p.Tk - 1)] != 0;
+                        const float v = allowed ? sc[4 * j + 2 * e + u] : -INFINITY;
+                        sc[4 * j + 2 * e + u] = v;
+                        mx = fmaxf(mx, v);
+                    }
                 }
             }
-            // the row's maximum over both column halves
-            bars->xchg[i & 1][half][row] = mx;
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            mx = fmaxf(mx, bars->xchg[i & 1][half ^ 1][row]);
-            const float m_new = fmaxf(m_run, mx);
-            const float m_use = (m_new == -INFINITY) ? 0.f : m_new;  // fully masked so far: every s is -inf, ex2(-inf - 0) = 0
-            float alpha;
-            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(alpha) : "f"(m_run - m_use));     // m_run = -inf -> 0 (o and l are 0 anyway)
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            const float m_new = fmaxf(m_run[e], mx);
+            const float m_use = (m_new == -INFINITY) ? 0.f : m_new;    // fully masked so far: every s is -inf, ex2(-inf - 0) = 0
+            alpha[e] = fa_ex2(m_run[e] - m_use);                        // m_run = -inf -> 0 (o and l are 0 anyway)
             float psum = 0.f;
-            unsigned ph[32], pl[32];
 #pragma unroll
-            for (int c = 0; c < 32; ++c) {
-                float pr;
-                asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(pr) : "f"(__uint_as_float(sv[c]) - m_use));
-                psum += pr;
-                const float hi = fa_rn_tf32(pr);
-                ph[c] = __float_as_uint(hi);
-                pl[c] = __float_as_uint(fa_rn_tf32(pr - hi));
+            for (int j = 0; j < 8; ++j) {
+#pragma unroll
+                for (int u = 0; u < 2; ++u) {
+                    const float pr = fa_ex2(sc[4 * j + 2 * e + u] - m_use);
+                    psum += pr;
+                    sc[4 * j + 2 * e + u] = pr;
+                }
             }
-            l_run = l_run * alpha + psum;
-            m_run = m_new;
-            // (the previous tile's PV MMA has been waited for below, so the P buffers are free)
-            fa_tmem_st32(tmem + lane_addr + FA_TM_PHI + col0, ph);
-            fa_tmem_st32(tmem + lane_addr + FA_TM_PLO + col0, pl);
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            asm volatile("{ .reg .b64 t; mbarrier.arrive.shared::cta.b64 t, [%0]; }" ::"r"(fa_s32(&bars->p_full)) : "memory");
-            // O <- O * alpha + P V   (this thread's 32 output dims)
-            ok = fa_wait(&bars->o_full, i & 1, err);
-            if (!ok) break;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            unsigned ov[32];
-            fa_tmem_ld32(ov, tmem + lane_addr + FA_TM_OT + col0);
-            fa_tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) o[j] = fmaf(o[j], alpha, __uint_as_float(ov[j]));
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+            l_run[e] = l_run[e] * alpha[e] + psum;                      // this thread's share of the row sum
+            m_run[e] = m_new;
         }
-        // row sum over both halves, then normalise; fully masked rows (left-pad queries) produce 0 like torch SDPA
-        bars->xchg[ntiles & 1][half][row] = l_run;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        const float l_tot = l_run + bars->xchg[ntiles & 1][half ^ 1][row];
-        if (q < p.Tq) {
-            const float inv = (ok && l_tot > 0.f) ? 1.0f / l_tot : 0.f;
-            float4* orow = reinterpret_cast<float4*>(p.o + (long long)b * p.o_bs + (long long)q * p.o_ld + h * FA_HD + col0);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) orow[j] = make_float4(o[4 * j] * inv, o[4 * j + 1] * inv, o[4 * j + 2] * inv, o[4 * j + 3] * inv);
+        for (int j = 0; j < 8; ++j) {
+            o[4 * j] *= alpha[0]; o[4 * j + 1] *= alpha[0]; o[4 * j + 2] *= alpha[1]; o[4 * j + 3] *= alpha[1];
+        }
+        // O += P V: k-step j covers keys 8 j .. 8 j + 7; A fragment (rows r, r + 8; columns tig, tig + 4) = keys 2 tig, 2 tig + 1 (VT order).
+        // The hi / lo fragments are all formed before the first MMA is issued, so the MMA batch runs without register hazards.
+        unsigned ph[8][4], pl[8][4];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int src[4] = {4 * j, 4 * j + 2, 4 * j + 1, 4 * j + 3};
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const float x = sc[src[u]], hi = fa_rn_tf32(x);
+                ph[j][u] = __float_as_uint(hi);
+                pl[j][u] = __float_as_uint(fa_rn_tf32(x - hi));
+            }
+        }
+        gmma_fence_regs(o);
+        gmma_fence();
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const unsigned vo = (j >> 2) * FA_KV_TILE + (j & 3) * 32;
+            const unsigned long long v_hi = gmma_desc(vb + vo), v_lo = gmma_desc(vb + 2 * FA_KV_TILE + vo);
+            gmma_m64n64k8_rs(o, ph[j], v_hi, 1u);
+            gmma_m64n64k8_rs(o, ph[j], v_lo, 1u);
+            gmma_m64n64k8_rs(o, pl[j], v_hi, 1u);
+        }
+        gmma_commit();
+        gmma_wait<0>();
+        gmma_fence_regs(o);
+        asm volatile("{ .reg .b64 t; mbarrier.arrive.shared::cta.b64 t, [%0]; }" ::"r"(fa_s32(&bars->kv_empty[s])) : "memory");
+    }
+    // row sums over the quad, then normalise; fully masked rows (left-pad queries) produce 0 like torch SDPA
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+        float l = l_run[e];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        if (qr[e] < p.Tq) {
+            const float inv = (ok && l > 0.f) ? 1.0f / l : 0.f;
+            float* orow = p.o + (long long)b * p.o_bs + (long long)qr[e] * p.o_ld + h * FA_HD + 2 * tig;
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(o[4 * j + 2 * e] * inv, o[4 * j + 2 * e + 1] * inv);
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(FA_TM_COLS) : "memory");
 }
 
 // q | k | v (token-major, strided) -> scaled tf32 hi / lo planes, head-major, V transposed; zero padded to whole tiles.
@@ -366,11 +309,12 @@ __global__ void __launch_bounds__(256) attn_prep_kernel(PrepParams p) {
             *reinterpret_cast<float4*>(dst) = hi;
             *reinterpret_cast<float4*>(dst + BH * p.Tk_pad * 64) = lo;
             const float yv[4] = {y.x, y.y, y.z, y.w};
+            const int col = (row & ~7) | ((row & 7) >> 1) | ((row & 1) << 2);      // key 2t -> column t, key 2t + 1 -> column t + 4
 #pragma unroll
             for (int c = 0; c < 4; ++c) {
                 const float vh = fa_rn_tf32(yv[c]);
-                vt_hi[d4 + c][row] = vh;
-                vt_lo[d4 + c][row] = fa_rn_tf32(yv[c] - vh);
+                vt_hi[d4 + c][col] = vh;
+                vt_lo[d4 + c][col] = fa_rn_tf32(yv[c] - vh);
             }
         }
     }
@@ -453,6 +397,7 @@ bool attn_tc_eligible(const AttentionParams& p, const AttnCtx* ctx) {
         (reinterpret_cast<uintptr_t>(p.o) & 15))
         return false;
     if ((p.q_bs % 4) || (p.k_bs % 4) || (p.v_bs % 4) || (p.o_bs % 4)) return false;
+    if ((p.q_ld % 4) || (p.k_ld % 4) || (p.v_ld % 4) || (p.o_ld % 4)) return false;      // float4 loads / float2 stores per row
     return true;
 }
 

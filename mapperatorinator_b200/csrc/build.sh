@@ -1,10 +1,10 @@
 #!/usr/bin/env bash
-# Builds libmapperatorinator_b200.so in-tree for sm_100a (cross-compiles without a GPU).
+# Builds libmapperatorinator_b200.so in-tree for sm_90a (H100; cross-compiles without a GPU).
 set -euo pipefail
 HERE="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 OUT="${HERE}/../libmapperatorinator_b200.so"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-FLAGS=(-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 --expt-relaxed-constexpr -Xcompiler -fPIC -Xcompiler -O3)
+FLAGS=(-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 --expt-relaxed-constexpr -Xcompiler -fPIC -Xcompiler -O3)
 if [[ "${MB200_PTXAS_V:-0}" == "1" ]]; then FLAGS+=(-Xptxas -v); fi
 mkdir -p "${HERE}/build"
 pids=()

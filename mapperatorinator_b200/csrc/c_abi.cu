@@ -68,14 +68,14 @@ extern "C" int mb200_op_gemm_tc(const float* A, int64_t lda, const float* W, int
     if (s) return s;
     if (!tc_gemm_eligible(g, ctx)) {
         ctx->unregister_weight(W);
-        MB_REQUIRE(false, "problem not eligible for the tcgen05 path (M >= 512, K % 4 == 0, 16-byte aligned operands)");
+        MB_REQUIRE(false, "problem not eligible for the wgmma path (M >= 512, K % 4 == 0, 16-byte aligned operands)");
     }
     s = launch_gemm_tc(g, (cudaStream_t)stream, ctx);
     cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream);
     ctx->unregister_weight(W);      // W belongs to the caller (a torch tensor whose address may be recycled)
     if (s) return s;
     MB_CUDA_CHECK(e);
-    MB_REQUIRE(ctx->error() == 0, "tcgen05 GEMM pipeline wait timed out");
+    MB_REQUIRE(ctx->error() == 0, "wgmma GEMM pipeline wait timed out");
     return 0;
 }
 
@@ -122,7 +122,7 @@ extern "C" int64_t mb200_audio_out_frames(int64_t n_frames, int32_t in_rate, int
 extern "C" int mb200_audio_ingest(const int16_t* pcm, int64_t n_frames, int32_t channels, int32_t in_rate, int32_t out_rate, int32_t normalize,
                                   float* out, int32_t* scratch, void* stream) {
     MB_REQUIRE(pcm && out && scratch, "null argument");
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     return mb200::launch_audio_ingest(reinterpret_cast<const short*>(pcm), (long long)n_frames, channels, in_rate, out_rate, normalize, out,
                                       reinterpret_cast<int*>(scratch), sms, (cudaStream_t)stream);

@@ -154,8 +154,8 @@ int launch_decode_attention(const DecAttnParams& p, cudaStream_t stream, bool pd
     if (p.rows <= 0) return 0;
     g_prof_class = 1;
     // Default: one CTA per unit with everything prefetched (the megakernel's phase body).  MB200_ATTN_BATCH=1 selects the
-    // one-warp-per-unit form for rows > 2 — the same arithmetic value for value (parity-tested), but measured SLOWER on B200
-    // (B = 64: 3.04 vs 3.30 TB/s, B = 8: 0.66 vs 1.15 TB/s): kept as the starting point for a persistent multi-unit kernel.
+    // one-warp-per-unit form for rows > 2 — the same arithmetic value for value (parity-tested), kept as the starting point for a
+    // persistent multi-unit kernel.
     static const int batch_form = [] { const char* e = getenv("MB200_ATTN_BATCH"); return e ? atoi(e) : 0; }();
     if (p.rows > 2 && batch_form) {
         const int units = p.rows * p.H * p.n_splits;

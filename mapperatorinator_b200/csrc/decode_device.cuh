@@ -244,7 +244,7 @@ __device__ __forceinline__ void gemv_row(const GemvParams& p, int n, const float
 
 // Merge of the split-KV partials, done ONCE per (row, head) by whichever split arrives last (threadfence-reduction pattern):
 // out[r, h*64+d] = sum_s w_s o_s[d] / sum_s w_s l_s, w_s = exp(m_s - max m), splits visited in index order, so the result does not
-// depend on which CTA happens to be last.  (It used to be a prologue of the following GEMV, i.e. all 148 CTAs re-did it, each
+// depend on which CTA happens to be last.  (It used to be a prologue of the following GEMV, i.e. every CTA re-did it, each
 // pulling every partial out of L2: 2-6 us per layer on the token's critical path.)
 __device__ __forceinline__ void decode_attention_merge(const DecAttnParams& p, int h, int r, float* stat, int tid) {
     // Arrival = ONE acq_rel atomic by thread 0 behind a CTA barrier (the same release/acquire shape as the grid barrier): the

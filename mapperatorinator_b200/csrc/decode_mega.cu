@@ -6,7 +6,7 @@
 // separated by a ~1 us grid barrier instead, and — because each CTA knows statically which weight rows it owns in the NEXT
 // GEMV phase — those rows are pulled into shared memory by the TMA bulk-copy engine (cp.async.bulk + mbarrier
 // complete_tx) while the current phase is still computing / waiting at its barrier.  HBM therefore streams weights
-// continuously across phase boundaries (2 x 77 KB in flight per SM, 148 SMs => ~22 MB outstanding), which is what the
+// continuously across phase boundaries (2 x 78 KB in flight per SM, 132 SMs => ~20 MB outstanding), which is what the
 // weight-streaming roofline needs; the math runs out of shared memory.
 //
 // Same arithmetic, same order as the per-kernel path (decode_device.cuh bodies are shared), so tokens are bit-identical.
@@ -58,7 +58,7 @@ __device__ __forceinline__ bool mbar_try_wait(unsigned long long* bar, unsigned 
                  : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
     return ok != 0;
 }
-// The 464 MB of decoder weights stream through the 126 MB L2 once per token.  With the default policy they evict everything
+// The 464 MB of decoder weights stream through the 50 MB L2 once per token.  With the default policy they evict everything
 // else — LayerNorm affine vectors, biases, phase descriptors, the K/V caches — so every small latency-critical load of the next
 // token misses to DRAM.  Tagging the weight stream evict-first keeps that small hot set resident in L2.
 __device__ __forceinline__ unsigned long long l2_evict_first_policy() {
@@ -76,6 +76,13 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
 __device__ __forceinline__ void cta_rows(int N, int cta, int rpc, int& r0, int& r1) {
     r0 = min(N, cta * rpc);
     r1 = min(N, r0 + rpc);
+}
+// Weight slice of a GEMV phase inside the two-buffer arena: buffer 0 starts at the front, buffer 1 ends at the back.  Consecutive GEMV
+// phases (always of opposite parity) therefore only need their two slices TOGETHER to fit the arena, which lets the vocabulary
+// projection's larger slice share it with its neighbours (mega_eligible in engine_model.cu checks every consecutive pair).
+// floats = rows per CTA x K of that phase.
+__device__ __forceinline__ float* wslice(float (&wbuf)[2][MEGA_WBUF_FLOATS], int buf, int floats) {
+    return buf ? &wbuf[0][0] + 2 * MEGA_WBUF_FLOATS - floats : &wbuf[0][0];
 }
 
 // thread 0: start streaming this CTA's weight rows of GEMV phase `ph` into wbuf[buf]
@@ -148,7 +155,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_megakernel(MegaParams 
     unsigned int sync_target = 0;
     if (tid == 0) {
         const MegaPhase* f = &mp.phases[mp.first_gemv];
-        prefetch_weights(f->g.W, f->g.ldw, f->g.N, f->g.K, sm.wbuf[0], &sm.mbar[0], cta, (f->g.N + G - 1) / G);
+        prefetch_weights(f->g.W, f->g.ldw, f->g.N, f->g.K, wslice(sm.wbuf, 0, 0), &sm.mbar[0], cta, (f->g.N + G - 1) / G);
     }
 
     // phase descriptors are double-buffered in shared memory: slot `cur` is the phase being executed, slot `cur ^ 1` is
@@ -240,11 +247,11 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_megakernel(MegaParams 
                     __syncthreads();
                 }
                 MEGA_TRACE(2);
-                // The next GEMV's weight slice is requested only now: measured on B200, issuing the ~5-9 MB bulk stream at
-                // the top of the phase queued this phase's few small latency-critical loads (activations, LN affine, bias)
-                // behind it and cost ~2.5 us per phase.  It still has the rest of this phase plus the next prologue to land.
+                // The next GEMV's weight slice is requested only now: issuing the ~5-9 MB bulk stream at the top of the phase
+                // queues this phase's few small latency-critical loads (activations, LN affine, bias) behind it.  It still has
+                // the rest of this phase plus the next prologue to land.
                 // issued by the LAST warp (it owns the fewest rows), from fields already in shared memory
-                if (tid == MEGA_THREADS - 32) prefetch_weights(ph.nx_W, ph.nx_ldw, ph.nx_N, ph.nx_K, sm.wbuf[buf ^ 1], &sm.mbar[buf ^ 1], cta, ph.nx_rpc);
+                if (tid == MEGA_THREADS - 32) prefetch_weights(ph.nx_W, ph.nx_ldw, ph.nx_N, ph.nx_K, wslice(sm.wbuf, buf ^ 1, ph.nx_rpc * ph.nx_K), &sm.mbar[buf ^ 1], cta, ph.nx_rpc);
                 wait_weights(&sm.mbar[buf], (g_idx >> 1) & 1, mp.error_flag);   // on a timeout the error flag ends the loop at the next token
                 MEGA_TRACE(3);
                 for (int rep = tracing ? 0 : 1; rep < 2; ++rep) {      // trace mode: a cold pass (stamp 12) and a warm one; idempotent, the
@@ -255,7 +262,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_megakernel(MegaParams 
                         const bool pre = j < OPS_ROWS;
                         const float bias_v = __shfl_sync(0xffffffffu, bias_pref, (j * MEGA_NB) & 31);
                         const float r_v = __shfl_sync(0xffffffffu, r_pref, (j * MEGA_NB + (lane < MEGA_NB ? lane : 0)) & 31);
-                        gemv_row<MEGA_NB, false>(ph.g, n, sm.wbuf[buf] + (long long)(n - r0) * ph.g.K, sm.u.xs, 0, lane, cur_pos, pre, bias_v, r_v,
+                        gemv_row<MEGA_NB, false>(ph.g, n, wslice(sm.wbuf, buf, ph.rpc * ph.g.K) + (long long)(n - r0) * ph.g.K, sm.u.xs, 0, lane, cur_pos, pre, bias_v, r_v,
                                                  (tracing && warp == 0 && rep == 1 && j == 0) ? &mp.trace[(long long)pi * MEGA_TRACE_SLOTS + 13] : nullptr);
                     }
                 }

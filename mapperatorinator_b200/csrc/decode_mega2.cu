@@ -13,7 +13,7 @@
 // is read by the 128 CTAs that own rows of the cross-q projection; the next writer of x, the cross out_proj, needs the merged cross
 // attention, which needs every row of cross-q).
 //
-// Structure of a CTA (148 CTAs x 256 threads x 255 registers, one per SM; DESIGN.md §4.1 has the measurements behind each choice):
+// Structure of a CTA (one CTA per SM x 256 threads x 255 registers; DESIGN.md §4.1 has the measurements behind each choice):
 //   * GEMV phases with a d_model-wide input (qkv, out, q_c, out_c, fc1, proj_out): threads 0..K/4-1 poll one float4 column each (pointers
 //     precomputed per thread), LayerNorm statistics over a named barrier of the polling warps, the activation is published in shared
 //     memory (the phase's one CTA barrier), then every warp takes whole weight rows with the activation in registers (gemv_dot's order)
@@ -91,6 +91,13 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
 __device__ __forceinline__ void cta_rows(int N, int cta, int rpc, int& r0, int& r1) {
     r0 = min(N, cta * rpc);
     r1 = min(N, r0 + rpc);
+}
+// Weight slice of a GEMV phase inside the two-buffer arena: buffer 0 starts at the front, buffer 1 ends at the back.  Consecutive GEMV
+// phases (always of opposite parity) therefore only need their two slices TOGETHER to fit the arena, which lets the vocabulary
+// projection's larger slice share it with its neighbours (mega_eligible in engine_model.cu checks every consecutive pair).
+// floats = rows per CTA x K of that phase.
+__device__ __forceinline__ float* wslice(float (&wbuf)[2][MEGA_WBUF_FLOATS], int buf, int floats) {
+    return buf ? &wbuf[0][0] + 2 * MEGA_WBUF_FLOATS - floats : &wbuf[0][0];
 }
 __device__ __forceinline__ void prefetch_weights(const float* W, long long ldw, int N, int K, float* dst, unsigned long long* bar, int cta, int rpc) {
     int r0, r1;
@@ -619,7 +626,7 @@ __device__ __forceinline__ void m3_rw_tail(const Mega2Params& mp, const Mega2Pha
 #pragma unroll
             for (int b = 0; b < NB; ++b) xr[b][j] = (j < nx && col < K4 && b < mp.rows) ? xs4[b * K4 + col] : make_float4(0, 0, 0, 0);
         }
-        const float4* wb4 = reinterpret_cast<const float4*>(sm.wbuf[buf]);
+        const float4* wb4 = reinterpret_cast<const float4*>(wslice(sm.wbuf, buf, ph.rpc * K));
         float4 acc[NB][4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
@@ -717,7 +724,7 @@ __device__ __forceinline__ void m3_gemv_phase(const Mega2Params& mp, const Mega2
     // it is done with it (a whole phase of lead for the copy).
     if (tid == M2_THREADS - 32) {
         if (g_idx > 0) wait_weights(&sm.wfree[buf ^ 1], ((g_idx - 1) >> 1) & 1, err);      // every warp has finished reading the slice of GEMV phase g_idx - 1
-        prefetch_weights(ph.nx_W, ph.nx_ldw, ph.nx_N, ph.nx_K, sm.wbuf[buf ^ 1], &sm.mbar[buf ^ 1], cta, ph.nx_rpc);
+        prefetch_weights(ph.nx_W, ph.nx_ldw, ph.nx_N, ph.nx_K, wslice(sm.wbuf, buf ^ 1, ph.nx_rpc * ph.nx_K), &sm.mbar[buf ^ 1], cta, ph.nx_rpc);
     }
     if (isd) {
         m3_rw_tail<NB>(mp, ph2, sm, cta, tid, buf, g_idx, par, in_tag, out_tag, cur_pos, err, trace, w, on, poller, in, r0, R);
@@ -868,7 +875,7 @@ __device__ __forceinline__ void m3_gemv_phase(const Mega2Params& mp, const Mega2
     // ---- multiply + reduce ----
     if (R > 0 && active_warp && !(c_ll_debug & 4)) {
         const int Pn = G == 1 ? R : (G == 2 ? (R + 1) >> 1 : (R + G - 1) / G);       // row slots per thread (host guarantees <= M3_SLOTS)
-        const float* wb = sm.wbuf[buf];
+        const float* wb = wslice(sm.wbuf, buf, ph.rpc * K);
         int kqc[M3_NS];
 #pragma unroll
         for (int s = 0; s < M3_NS; ++s) kqc[s] = kq0 + s * M2_THREADS < K4 ? kq0 + s * M2_THREADS : 0;
@@ -936,7 +943,7 @@ __global__ void __launch_bounds__(M2_THREADS, 1) decode_megakernel_ll(Mega2Param
     unsigned int g_idx = 0;          // running index of GEMV phases (selects weight buffer + mbarrier parity)
     if (tid == 0) {
         const MegaPhase* f = &mp.phases[0].base;
-        prefetch_weights(f->g.W, f->g.ldw, f->g.N, f->g.K, sm.wbuf[0], &sm.mbar[0], cta, (f->g.N + G - 1) / G);
+        prefetch_weights(f->g.W, f->g.ldw, f->g.N, f->g.K, wslice(sm.wbuf, 0, 0), &sm.mbar[0], cta, (f->g.N + G - 1) / G);
     }
     // CTA 0 publishes the residual stream left by the prefill (plain memory, written by an earlier kernel) and the first token header
     // under the tag the first phase of step 0 expects: "last phase of step -1"

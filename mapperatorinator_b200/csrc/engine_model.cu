@@ -829,9 +829,13 @@ static bool mega_eligible(const mb200_model* m, int rows) {
     if (!m->use_mega || rows > 2 || m->num_sms <= 0) return false;
     const auto& c = m->cfg;
     const int G = m->num_sms;
-    auto fits = [&](int N, int K) { return (size_t)((N + G - 1) / G) * K <= (size_t)MEGA_WBUF_FLOATS; };
-    return c.ffn_dim <= 3072 && fits(3 * c.d_model, c.d_model) && fits(c.d_model, c.d_model) && fits(c.ffn_dim, c.d_model) &&
-           fits(c.d_model, c.ffn_dim) && fits(c.vocab_size_out, c.d_model);
+    // per-CTA weight slices of the token's GEMV phases; consecutive phases (qkv, out, cross q, cross out, fc1, fc2 per layer, then
+    // the vocabulary projection, then the next token's qkv) share the two-buffer arena from opposite ends
+    auto slice = [&](int N, int K) { return (size_t)((N + G - 1) / G) * K; };
+    const int d = c.d_model, f = c.ffn_dim;
+    const size_t qkv = slice(3 * d, d), dd = slice(d, d), fc1 = slice(f, d), fc2 = slice(d, f), voc = slice(c.vocab_size_out, d);
+    auto pair = [&](size_t a, size_t b) { return a + b <= (size_t)2 * MEGA_WBUF_FLOATS; };
+    return f <= 3072 && pair(qkv, dd) && pair(dd, dd) && pair(dd, fc1) && pair(fc1, fc2) && pair(fc2, qkv) && pair(fc2, voc) && pair(voc, qkv);
 }
 
 static SampleConfig make_sample_config(const mb200_generate_params* gp, int B, bool use_cfg, int V, int ids_ld) {

@@ -1,18 +1,18 @@
-// Tensor-core GEMM for the dense phases (encoder layers, conv stem, DiT blocks): tcgen05.mma kind::tf32 with fp32-grade
-// accuracy through the 3xTF32 split
+// Tensor-core GEMM for the dense phases (encoder layers, conv stem, DiT blocks): Hopper wgmma (kind tf32) with fp32-grade accuracy
+// through the 3xTF32 split
 //        A.W^T  ~=  Ahi.Whi^T + Ahi.Wlo^T + Alo.Whi^T ,   x = xhi + xlo,  xhi = rn_tf32(x), xlo = rn_tf32(x - xhi).
 // Both parts are rounded to nearest tf32 (cvt.rna) — weights once at load, activations by a tiny elementwise pass — because the
-// tensor core would otherwise TRUNCATE the low 13 bits, and truncation bias adds up linearly over K.  Accumulation is fp32 in TMEM.  Measured error vs fp64 is ~1e-6 relative — the same order as an fp32 FMA chain of that
-// length — which is what bit-exact greedy decoding against the fp32 reference needs; plain TF32 (1e-3) flips tokens.
+// tensor core would otherwise TRUNCATE the low 13 bits, and truncation bias adds up linearly over K.  Accumulation is fp32 in registers.
+// The error vs fp64 is ~1e-6 relative — the same order as an fp32 FMA chain of that length — which is what bit-exact greedy decoding
+// against the fp32 reference needs; plain TF32 (1e-3) flips tokens.
 //
-// Structure (one 128x128 output tile per CTA, 192 threads):
-//   warp 0 / lane 0 : TMA producer — 4 tiles per k-block (A, Alo, W, Wlo; 128 rows x 32 floats, SWIZZLE_128B) into a 3-stage ring
-//   warp 1 / lane 0 : MMA issuer   — 12 x tcgen05.mma (128x128x8) per k-block into a 128-column fp32 TMEM accumulator,
-//                     tcgen05.commit frees the stage / publishes the accumulator
-//   warps 2..5      : epilogue     — tcgen05.ld (32 lanes x 32 columns per warp and pass) -> per-warp shared-memory transpose ->
-//                     bias / activation / gate / residual (same GemmParams epilogue as gemm.cu) -> 128-byte coalesced stores
-// Measured alternative (kept out): deriving hi/lo inside the kernel from raw tiles (half the L2->SM operand traffic, no mirror
-// copies) was 10-15 % SLOWER — the split's shared-memory traffic competes with the MMA's own operand reads.
+// Structure (one 128x128 output tile per CTA, 384 threads = 3 warpgroups):
+//   warpgroup 0, thread 0 : TMA producer — 4 tiles per k-block (A, Alo, W, Wlo; 128 rows x 32 floats, SWIZZLE_128B) into a 3-stage ring
+//   warpgroups 1, 2       : MMA + epilogue — warpgroup g owns output rows 64(g-1) .. +63: 12 x wgmma m64n128k8 per k-block into a
+//                           64-register fp32 accumulator per thread; the stage is released (mbarrier, every consumer thread arrives)
+//                           once the warpgroup's MMAs have completed.  Epilogue: accumulators -> shared memory (the idle pipeline
+//                           stages) -> row by row with lane = column: bias / activation / gate / residual (same GemmParams epilogue
+//                           as gemm.cu) and 128-byte coalesced loads and stores.
 // A may be any RowMap (im2col-free conv over the padded buffer, batched rows) via a 3-D tensor map.
 // Every wait is bounded: on a timeout the kernel sets an error flag and falls through, it can never hang the GPU.
 #include <cuda.h>
@@ -27,6 +27,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace mb200 {
 
@@ -34,16 +35,15 @@ int g_tc_enabled = 1;
 
 namespace {
 
-constexpr int TC_BM = 128, TC_BN = 128, TC_BK = 32, TC_STAGES = 3, TC_THREADS = 192;
+constexpr int TC_BM = 128, TC_BN = 128, TC_BK = 32, TC_STAGES = 3, TC_THREADS = 384, TC_CONSUMERS = 256;
 constexpr int TC_TILE_BYTES = TC_BM * TC_BK * 4;          // 16 KB
 constexpr int TC_STAGE_BYTES = 4 * TC_TILE_BYTES;         // A, Alo, W, Wlo
+constexpr int TC_EPI_LD = TC_BN + 8;                      // epilogue staging row (floats): the fragment's float2 stores are conflict-free
+static_assert(TC_BM * TC_EPI_LD * 4 <= TC_STAGES * TC_STAGE_BYTES, "epilogue staging fits the pipeline stages");
 
 struct TcBarriers {
     unsigned long long full[TC_STAGES];
     unsigned long long empty[TC_STAGES];
-    unsigned long long tmem_full;
-    unsigned int tmem_base;
-    int pad;
 };
 
 __device__ __forceinline__ unsigned s32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -59,78 +59,37 @@ __device__ __forceinline__ bool bar_wait(unsigned long long* bar, unsigned parit
     return false;
 }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 | LBO=1 | SBO=1024B>>4 | version 1 | layout 2
-__device__ __forceinline__ unsigned long long umma_desc(unsigned smem_addr) {
-    unsigned long long d = 0;
-    d |= (unsigned long long)((smem_addr >> 4) & 0x3FFF);
-    d |= (unsigned long long)1 << 16;
-    d |= (unsigned long long)(1024 >> 4) << 32;
-    d |= (unsigned long long)1 << 46;
-    d |= (unsigned long long)2 << 61;
-    return d;
-}
-
-__device__ __forceinline__ void umma_tf32(unsigned tmem_d, unsigned long long da, unsigned long long db, unsigned idesc, unsigned accumulate) {
-    asm volatile("{ .reg .pred p; setp.ne.b32 p, %4, 0; tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p; }"
-                 ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-__device__ __forceinline__ void umma_commit(unsigned long long* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"l"(__cvta_generic_to_shared(bar)) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(unsigned (&v)[32], unsigned taddr) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, "
-        "%20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_alo,
                    const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo, GemmParams p, int a_rpb, int* err) {
     extern __shared__ unsigned char tc_smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~uintptr_t(1023));
     TcBarriers* bars = reinterpret_cast<TcBarriers*>(smem + TC_STAGES * TC_STAGE_BYTES);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x;
     const int n0 = blockIdx.x * TC_BN;
     const long long m0 = (long long)blockIdx.y * TC_BM;
     const int nkb_all = (p.K + TC_BK - 1) / TC_BK;
     // Split-K (kernels.h): k-range z = k-blocks [z*kpb, (z+1)*kpb) is summed on its own.  Grid split (under-filled grids): CTA
     // blockIdx.z owns range z and stores raw partials, gemm.cu's reduce kernel adds them in order.  In-tile split (large M): this CTA
-    // walks every range, range z accumulating into TMEM columns [z*128, z*128+128); the epilogue adds the S accumulators in the same
-    // order.  Same partial sums, same additions, same bits.
+    // walks every range, each range accumulating from zero; the running sum adds the range results in the same order.  Same
+    // partial sums, same additions, same bits.
     const int kpb = p.splitk > 1 ? p.k_per_split / TC_BK : nkb_all;
     const bool grid_split = p.split_mode == 1, tile_split = p.split_mode == 2;
     const int kb0 = grid_split ? blockIdx.z * kpb : 0;
     const int nkb = grid_split ? max(0, min(nkb_all - kb0, kpb)) : nkb_all;
-    const int nacc = tile_split ? p.splitk : 1;
-    const unsigned tmem_cols = nacc == 1 ? 128u : (nacc == 2 ? 256u : 512u);
 
     if (tid == 0) {
         for (int s = 0; s < TC_STAGES; ++s) {
             asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(s32(&bars->full[s])));
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(s32(&bars->empty[s])));
+            asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(&bars->empty[s])), "r"(TC_CONSUMERS));
         }
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(s32(&bars->tmem_full)));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(&bars->tmem_base)), "r"(tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const unsigned tmem = bars->tmem_base;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (tid < 128) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");      // the producer needs few registers; the accumulators get them
+        if (tid == 0) {
             const int a_b = a_rpb > 0 ? (int)(m0 / a_rpb) : 0;
             const int a_t = a_rpb > 0 ? (int)(m0 - (long long)a_b * a_rpb) : (int)m0;
             for (int kb = 0; kb < nkb; ++kb) {
@@ -151,117 +110,94 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
                              ::"r"(s32(st + 3 * TC_TILE_BYTES)), "l"(&map_wlo), "r"(k0), "r"(n0), "r"(fb) : "memory");
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // instruction descriptor (cute::UMMA::InstrDescriptor): D fp32, A/B tf32, both K-major, N = 128, M = 128
-            const unsigned idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((unsigned)(TC_BN >> 3) << 17) | ((unsigned)(TC_BM >> 4) << 24);
-            bool ok = true;
-            for (int kb = 0; kb < nkb && ok; ++kb) {
-                const int s = kb % TC_STAGES;
-                const unsigned ph = (kb / TC_STAGES) & 1;
-                ok = bar_wait(&bars->full[s], ph, err);
-                if (!ok) break;
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const unsigned base = s32(smem + s * TC_STAGE_BYTES);
-                const int z = tile_split ? kb / kpb : 0, kr = tile_split ? kb - z * kpb : kb;      // accumulator and position inside its k-range
-                const unsigned acc = tmem + (unsigned)(z * TC_BN);
+        return;      // the bulk copies in flight complete on the mbarriers of this (still resident) CTA
+    }
+
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int ct = tid - 128;                          // consumer thread 0..255
+    const int cg = ct >> 7;                            // consumer warpgroup: output rows 64 cg .. +63
+    float acc[64], sum[64];
 #pragma unroll
-                for (int sub = 0; sub < TC_BK / 8; ++sub) {
-                    const unsigned off = sub * 32;       // 8 tf32 = 32 bytes along K inside the 128-byte swizzle atom
-                    const unsigned long long a_hi = umma_desc(base + off), a_lo = umma_desc(base + TC_TILE_BYTES + off);
-                    const unsigned long long w_hi = umma_desc(base + 2 * TC_TILE_BYTES + off), w_lo = umma_desc(base + 3 * TC_TILE_BYTES + off);
-                    umma_tf32(acc, a_hi, w_hi, idesc, (kr > 0 || sub > 0) ? 1u : 0u);
-                    umma_tf32(acc, a_hi, w_lo, idesc, 1u);
-                    umma_tf32(acc, a_lo, w_hi, idesc, 1u);
-                }
-                umma_commit(&bars->empty[s]);            // frees the stage once these MMAs have read it
-            }
-            umma_commit(&bars->tmem_full);               // accumulator complete
-        }
-    } else {
-        const bool ok = true;                             // (the wait for the accumulator comes after the first operand prefetch, below)
-        const int lg = warp & 3;                          // TMEM lane group this warp may access
-        static_assert(sizeof(TcBarriers) <= 256, "barrier block");
-        // Epilogue: tcgen05.ld hands every thread 32 consecutive columns of ITS row, so storing straight from registers would make
-        // each store instruction touch 32 different rows (32 sectors per instruction; measured: the epilogue, not the MMA pipe,
-        // set the kernel's duration).  Each warp transposes its 32x32 block through shared memory instead (the pipeline stages
-        // are idle by now: every TMA load and every MMA that reads them completed before tmem_full fired) and then walks the
-        // block row by row with lane = column: bias / gate / residual loads and the C store are all 128-byte coalesced.
-        float* stg = reinterpret_cast<float*>(smem) + lg * (32 * 33);                    // [32 rows][33] per warp
-        struct RowPtrs { float* c; const float* r; const float* g; };
-        // (its own shared-memory region behind the barriers: it is written while the main loop still owns the pipeline stages)
-        RowPtrs* rows = reinterpret_cast<RowPtrs*>(smem + TC_STAGES * TC_STAGE_BYTES + 256) + lg * 32;  // this warp's 32 row bases
-        {
-            const long long m = m0 + lg * 32 + lane;
-            RowPtrs rp{nullptr, nullptr, nullptr};
-            if (ok && m < p.M) {
-                if (grid_split) {
-                    rp.c = p.splitk_ws + ((long long)blockIdx.z * p.M + m) * p.N;         // raw partial sums of this split
-                } else {
-                    rp.c = p.C.row(m);
-                    rp.r = p.R.ptr ? p.R.row(m) : nullptr;
-                    rp.g = p.gate ? p.gate + (m / p.gate_rpb) * p.gate_ld : nullptr;
-                }
-            }
-            rows[lane] = rp;
-        }
-        __syncwarp();
-        // Residual / gate operands of a 32-column chunk do not depend on the accumulator: all 32 rows' loads are issued in one batch
-        // BEFORE the chunk's TMEM read (chunk 0: before the accumulator is even complete — the epilogue warps idle through the main
-        // loop), instead of one dependent L2 round trip per row behind the transpose (ncu: 20 % of the kernel's samples sat on those loads).
-        const bool has_r = !grid_split && p.R.ptr != nullptr, has_g = !grid_split && p.gate != nullptr;
-        float rv[32], gv[32];
-        auto fetch_rg = [&](int c0) {
-            const int n = n0 + c0 + lane;
-            const bool n_ok = n < p.N;
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) {
-                const RowPtrs rp = rows[rr];
-                rv[rr] = (has_r && n_ok && rp.r) ? rp.r[n] : 0.f;
-                gv[rr] = (has_g && n_ok && rp.g) ? __ldg(rp.g + n) : 1.f;
-            }
-        };
-        if (has_r || has_g) fetch_rg(0);
-        const bool ok2 = bar_wait(&bars->tmem_full, 0, err);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        (void)ok2;
+    for (int i = 0; i < 64; ++i) { acc[i] = 0.f; sum[i] = 0.f; }
 #pragma unroll 1
-        for (int c0 = 0; c0 < TC_BN; c0 += 32) {
-            unsigned v[32];
-            const unsigned taddr = tmem + ((unsigned)(lg * 32) << 16) + (unsigned)c0;
-            tmem_ld32(v, taddr);
-            for (int z = 1; z < nacc; ++z) {                                              // in-tile split: ((acc0 + acc1) + acc2) + acc3
-                unsigned w[32];
-                tmem_ld32(w, taddr + (unsigned)(z * TC_BN));
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int s = kb % TC_STAGES;
+        const unsigned ph = (kb / TC_STAGES) & 1;
+        if (!bar_wait(&bars->full[s], ph, err)) break;
+        const unsigned base = s32(smem + s * TC_STAGE_BYTES);
+        const unsigned a_off = (unsigned)cg * (64 * 128);                                 // 64 rows of 128 bytes
+        const int z = tile_split ? kb / kpb : 0, kr = tile_split ? kb - z * kpb : kb;      // k-range and position inside it
+        gmma_fence_regs(acc);
+        gmma_fence();
 #pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(w[j]));
+        for (int sub = 0; sub < TC_BK / 8; ++sub) {
+            const unsigned off = sub * 32;       // 8 tf32 = 32 bytes along K inside the 128-byte swizzle atom
+            const unsigned long long a_hi = gmma_desc(base + a_off + off), a_lo = gmma_desc(base + TC_TILE_BYTES + a_off + off);
+            const unsigned long long w_hi = gmma_desc(base + 2 * TC_TILE_BYTES + off), w_lo = gmma_desc(base + 3 * TC_TILE_BYTES + off);
+            gmma_m64n128k8_ss(acc, a_hi, w_hi, (kr > 0 || sub > 0) ? 1u : 0u);
+            gmma_m64n128k8_ss(acc, a_hi, w_lo, 1u);
+            gmma_m64n128k8_ss(acc, a_lo, w_hi, 1u);
+        }
+        gmma_commit();
+        gmma_wait<0>();
+        gmma_fence_regs(acc);
+        asm volatile("{ .reg .b64 t; mbarrier.arrive.shared::cta.b64 t, [%0]; }" ::"r"(s32(&bars->empty[s])) : "memory");
+        if (kb == nkb - 1 || (tile_split && kr == kpb - 1)) {                            // a k-range is complete: ((r0 + r1) + r2) + r3
+            if (z == 0) {
+#pragma unroll
+                for (int i = 0; i < 64; ++i) sum[i] = acc[i];
+            } else {
+#pragma unroll
+                for (int i = 0; i < 64; ++i) sum[i] += acc[i];
             }
-#pragma unroll
-            for (int j = 0; j < 32; ++j) stg[lane * 33 + j] = __uint_as_float(v[j]);     // bank (lane + j) % 32: conflict-free
-            __syncwarp();
-            const int n = n0 + c0 + lane;
-            const bool n_ok = n < p.N;
-            const float bias_v = (n_ok && p.bias) ? __ldg(p.bias + n) : 0.f;
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) {
-                const RowPtrs rp = rows[rr];                                              // broadcast
-                if (rp.c && n_ok) {
-                    float x = stg[rr * 33 + lane];
-                    if (grid_split) { rp.c[n] = x; continue; }
-                    if (p.bias) x += bias_v;
-                    x = apply_act(x, p.act) * p.alpha;
-                    if (has_g) x *= gv[rr];
-                    if (has_r) x += rv[rr];
-                    rp.c[n] = x;
-                }
-            }
-            __syncwarp();                                                                 // block consumed before the next chunk overwrites it
-            if ((has_r || has_g) && c0 + 32 < TC_BN) fetch_rg(c0 + 32);                   // next chunk's operands travel while its TMEM read / transpose run
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tmem_cols) : "memory");
+
+    // Epilogue.  Both consumer warpgroups are past their last MMA (every TMA load they waited for has landed), so the pipeline
+    // stages are free: the tile goes through shared memory [128][TC_EPI_LD] and is then walked row by row with lane = column.
+    asm volatile("bar.sync 1, %0;" ::"n"(TC_CONSUMERS) : "memory");
+    float* stg = reinterpret_cast<float*>(smem);
+    {
+        const int w = (ct >> 5) & 3, lane = ct & 31, gid = lane >> 2, tig = lane & 3;
+        const int r = cg * 64 + w * 16 + gid;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const int c = 8 * j + 2 * tig;
+            *reinterpret_cast<float2*>(stg + r * TC_EPI_LD + c) = make_float2(sum[4 * j], sum[4 * j + 1]);
+            *reinterpret_cast<float2*>(stg + (r + 8) * TC_EPI_LD + c) = make_float2(sum[4 * j + 2], sum[4 * j + 3]);
+        }
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(TC_CONSUMERS) : "memory");
+    const int lane = ct & 31, cw = ct >> 5;            // consumer warp cw stores rows 16 cw .. +15
+    const bool has_r = !grid_split && p.R.ptr != nullptr, has_g = !grid_split && p.gate != nullptr;
+    float bias_v[TC_BN / 32];
+#pragma unroll
+    for (int c = 0; c < TC_BN / 32; ++c) {
+        const int n = n0 + 32 * c + lane;
+        bias_v[c] = (!grid_split && p.bias && n < p.N) ? __ldg(p.bias + n) : 0.f;
+    }
+#pragma unroll 1
+    for (int rr = 0; rr < 16; ++rr) {
+        const int row = cw * 16 + rr;
+        const long long m = m0 + row;
+        if (m >= p.M) break;
+        float* crow = grid_split ? p.splitk_ws + ((long long)blockIdx.z * p.M + m) * p.N : p.C.row(m);
+        const float* rrow = has_r ? p.R.row(m) : nullptr;
+        const float* grow = has_g ? p.gate + (m / p.gate_rpb) * p.gate_ld : nullptr;
+#pragma unroll
+        for (int c = 0; c < TC_BN / 32; ++c) {
+            const int n = n0 + 32 * c + lane;
+            if (n >= p.N) continue;
+            float x = stg[row * TC_EPI_LD + 32 * c + lane];
+            if (!grid_split) {
+                if (p.bias) x += bias_v[c];
+                x = apply_act(x, p.act) * p.alpha;
+                if (has_g) x *= __ldg(grow + n);
+                if (has_r) x += rrow[n];
+            }
+            crow[n] = x;
+        }
+    }
 }
 
 // x = hi + lo with hi = round-to-nearest tf32(x) and lo = round-to-nearest tf32(x - hi).  Rounding (not truncating) both parts
@@ -315,7 +251,7 @@ int make_map(CUtensorMap* out, const float* base, long long K, long long rows_pe
 }  // namespace
 
 // S of an (N, K) problem on the tensor-core path: the split that fills the machine for ONE encoder window (M = 512 rows = 4 row
-// tiles), at least 8 k-blocks per range, at most 4 ranges (4 x 128 TMEM columns).  A function of N and K only.
+// tiles), at least 8 k-blocks per range, at most 4 ranges.  A function of N and K only.
 int gemm_splits_tc(int N, int K, int num_sms, int* k_per_split) {
     const int tiles_ref = 4 * ((N + TC_BN - 1) / TC_BN), nkb = (K + TC_BK - 1) / TC_BK;
     int splits = std::max(1, std::min({4, num_sms / std::max(1, tiles_ref), nkb / 8}));
@@ -326,7 +262,7 @@ int gemm_splits_tc(int N, int K, int num_sms, int* k_per_split) {
 }
 
 // One-time self test of the tensor-core path against a host fp64 product (grid split, in-tile split and unsplit shapes).  If the
-// tcgen05 pipeline misbehaves on this driver / device the path is switched off LOUDLY and every GEMM stays on the fp32 SIMT kernel.
+// wgmma pipeline misbehaves on this driver / device the path is switched off LOUDLY and every GEMM stays on the fp32 SIMT kernel.
 static int g_tc_tested = 0;
 static void tc_self_test() {
     g_tc_tested = 1;
@@ -370,7 +306,7 @@ static void tc_self_test() {
     ctx.destroy();
     if (!all_ok) {
         g_tc_enabled = 0;
-        fprintf(stderr, "[mapperatorinator_b200] WARNING: tcgen05 GEMM self-test FAILED — tensor-core path disabled, using the fp32 SIMT GEMM\n");
+        fprintf(stderr, "[mapperatorinator_b200] WARNING: wgmma GEMM self-test FAILED — tensor-core path disabled, using the fp32 SIMT GEMM\n");
         cudaGetLastError();
     }
 }
@@ -419,7 +355,7 @@ int launch_gemm_tc(const GemmParams& p, cudaStream_t stream, GemmCtx* ctx) {
     MB_REQUIRE(make_map(&mw, wm.hi, p.K, p.N, p.ldw, 1, 0, 2) == 0, "tensor map Whi");
     MB_REQUIRE(make_map(&mwl, wm.lo, p.K, p.N, p.ldw, 1, 0, 2) == 0, "tensor map Wlo");
     static bool configured = false;
-    const int smem = TC_STAGES * TC_STAGE_BYTES + 256 + 4 * 32 * 24 + 1024;      // stages | barriers (256 B) | epilogue row table | alignment slack
+    const int smem = TC_STAGES * TC_STAGE_BYTES + (int)sizeof(TcBarriers) + 1024;      // stages | barriers | alignment slack
     if (!configured) {
         MB_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         configured = true;

@@ -25,7 +25,7 @@ struct GemmParams {
     // S partial sums are added in index order.  HOW the partials are realised is a launch decision that does not change a bit:
     //   split_mode 1 ("grid"):    CTA z = blockIdx.z writes raw partials to ws[z][M][N]; gemm_splitk_reduce_kernel adds them in order
     //                             and applies the epilogue (under-filled grids);
-    //   split_mode 2 ("in-tile"): one CTA walks all of K with S accumulators (tcgen05 path: S x 128 TMEM columns) and its epilogue
+    //   split_mode 2 ("in-tile"): one CTA walks all of K with S accumulators (tensor-core path: one range at a time, a running sum in registers) and its epilogue
     //                             adds them in the same order (large M).
     float* splitk_ws; int splitk; int k_per_split; int split_mode;
     long long m_base;       // logical row of local row 0 (launch_gemm slices M when the partial planes of a grid split exceed the workspace)
@@ -35,9 +35,9 @@ struct GemmParams {
 // engines on two streams raced on them, and a reallocation could pull memory from under a captured CUDA graph).
 struct Tf32Mirror { const float* hi; const float* lo; };
 struct GemmCtx {
-    int num_sms = 148;
+    int num_sms = 132;
     float* splitk_ws = nullptr; size_t splitk_bytes = 0;        // [S][M][N] partial sums of the grid split
-    float* a_split = nullptr; size_t a_split_bytes = 0;         // tf32 hi | lo copies of the activation operand (tcgen05 path)
+    float* a_split = nullptr; size_t a_split_bytes = 0;         // tf32 hi | lo copies of the activation operand (tensor-core path)
     int* tc_err = nullptr;                                      // device flag: 0 fine, 3 = a pipeline wait timed out
     bool frozen = false;                                        // set once a CUDA graph holds these pointers: reserve() may no longer move them
     std::unordered_map<const float*, Tf32Mirror> mirrors;       // weight matrix -> its tf32 hi / lo arrays (filled at finalize)
@@ -49,7 +49,7 @@ struct GemmCtx {
 };
 GemmCtx* default_gemm_ctx();                                    // scratch of the kernel-level test entry points (mb200_op_gemm*)
 int launch_gemm(const GemmParams& p, cudaStream_t stream, GemmCtx* ctx);
-// gemm_tc.cu — tcgen05 3xTF32 path (fp32-grade accuracy on the tensor cores); launch_gemm dispatches to it for large problems
+// gemm_tc.cu — wgmma 3xTF32 path (fp32-grade accuracy on the tensor cores); launch_gemm dispatches to it for large problems
 // whose weight matrix has a registered tf32 "lo" mirror
 extern int g_tc_enabled;
 int launch_splitk_reduce(const GemmParams& q, cudaStream_t stream);
@@ -101,7 +101,7 @@ extern int g_attn_tc_enabled, g_attn_tc_min_t;
 size_t attn_tc_workspace_bytes(int B, int H, int Tq, int Tk);
 bool attn_tc_eligible(const AttentionParams& p, const AttnCtx* ctx);
 int launch_attention_tc(const AttentionParams& p, cudaStream_t stream, AttnCtx* ctx);
-// ctx != null and an eligible problem (no dense mask, no kv_slot gather, enough queries): tcgen05 flash attention; else the fp32 SIMT kernel
+// ctx != null and an eligible problem (no dense mask, no kv_slot gather, enough queries): wgmma flash attention; else the fp32 SIMT kernel
 int launch_attention(const AttentionParams& p, cudaStream_t stream, AttnCtx* ctx = nullptr);
 
 // ---- slider.cu: slider end-point recompute of the diffusion denoised_fn (diffusion_pipeline.py:203-222) -------------------
@@ -240,7 +240,7 @@ struct SampleParams {
 int launch_sample(const SampleParams& p, int B, cudaStream_t stream, bool pdl);
 
 // ---- decode_mega.cu: the persistent token-loop megakernel ----------------------------------------------------------------
-constexpr int MEGA_WBUF_FLOATS = 19712;       // 77 KB weight slice per buffer (two buffers per CTA)
+constexpr int MEGA_WBUF_FLOATS = 19968;       // 78 KB per buffer, two buffers per CTA (one arena: see wslice in decode_mega.cu)
 struct MegaPhase {                            // one dependent micro-phase of a token (built on the host)
     int kind;                                 // 0 GEMV, 1 split-KV attention, 2 logits chain + token selection
     int next_gemv;                            // index of the next GEMV phase (wraps into the next token)
@@ -278,8 +278,8 @@ struct MegaLL {                                   // engine-owned exchange buffe
     unsigned long long* part;                     // [rows][H][max_splits][66]  split-KV partials: o[64], m, l
     unsigned long long* hdr;                      // [0] cur_len, [1] all_finished of the NEXT token (written by the selection phase)
     int max_splits;
-    // x, att and h are read by (almost) every CTA.  148 SMs polling the same 6 KB turned its L2 lines into a hot spot (measured: the
-    // tagged stores took ~3 us to become visible under that read pressure), so these three buffers exist `reps` times; producers store
+    // x, att and h are read by (almost) every CTA.  Every SM polling the same 6 KB turns its L2 lines into a hot spot (the tagged
+    // stores become visible late under that read pressure), so these three buffers exist `reps` times; producers store
     // every replica, CTA c polls replica c % reps.
     int reps;
     long long x_rep, h_rep;                       // replica strides of x / att (2 * d) and h (2 * ffn), in pairs

@@ -68,7 +68,7 @@ class ModelEngine:
     def __init__(self, cfg: ModelConfig, state_dict: Dict[str, torch.Tensor], max_windows: int = 32, max_batch: int = 16,
                  mel_basis: Optional[np.ndarray] = None, device: str = "cuda:0"):
         if not torch.cuda.is_available():
-            raise RuntimeError("mapperatorinator_b200 needs a CUDA device (sm_100a); there is no CPU path")
+            raise RuntimeError("mapperatorinator_b200 needs a CUDA device (sm_90a); there is no CPU path")
         self.cfg = cfg
         self.device = torch.device(device)
         self.lib = _lib.load()
@@ -233,7 +233,7 @@ class DiTEngine:
     def __init__(self, cfg: DiTConfig, state_dict: Dict[str, torch.Tensor], max_seq_len: int = 1024, max_batch: int = 2,
                  device: str = "cuda:0"):
         if not torch.cuda.is_available():
-            raise RuntimeError("mapperatorinator_b200 needs a CUDA device (sm_100a); there is no CPU path")
+            raise RuntimeError("mapperatorinator_b200 needs a CUDA device (sm_90a); there is no CPU path")
         self.cfg = cfg
         self.device = torch.device(device)
         self.lib = _lib.load()

@@ -37,7 +37,7 @@ def gemm(a, w, bias=None, act="none", alpha=1.0, residual=None, gate=None, gate_
 
 
 def gemm_tc(a, w, bias=None, act="none", alpha=1.0, residual=None):
-    """Same contract as `gemm`, forced through the tcgen05 3xTF32 kernel."""
+    """Same contract as `gemm`, forced through the wgmma 3xTF32 kernel."""
     lib = _lib.load()
     a, w = _f32c(a), _f32c(w)
     M, K = a.shape

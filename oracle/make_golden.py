@@ -1,6 +1,6 @@
-"""Generate tests/golden/*.npz from the UNMODIFIED reference classes (run in the build container: needs /root/reference).
+"""Generate tests/golden/*.npz from the UNMODIFIED reference classes (needs a checkout of the original Mapperatorinator project).
 
-TEST INFRASTRUCTURE.  Usage:  python -m oracle.make_golden
+TEST INFRASTRUCTURE.  Usage:  MAPPERATORINATOR_REFERENCE=<checkout of the original project> python -m oracle.make_golden
 Inputs are regenerated from seeds by the tests (torch CPU generator); only reference OUTPUTS are stored.
 Weights are `init_model_state_dict(cfg, seed)` loaded into the reference model with `load_state_dict`, so no checkpoint
 is stored either.  Every case records the library versions the outputs were produced with.
@@ -62,11 +62,7 @@ def main():
             ids, stats = model_generate(model, tok2, dict(mk), dict(gk))
             gen_out[f"{flavour}/{cname}/ids"] = ids.numpy()
             gen_out[f"{flavour}/{cname}/counts"] = np.array(stats["generated_tokens_per_sample"])
-        if flavour == "torchaudio":                               # long prompts: decoder-side only, one flavour is enough
-            for cname, (prompt, gk, seed) in cases.long_context_cases().items():
-                mk = dict(inputs=cases.model_pcm(cfg, prompt.shape[0], seed), decoder_input_ids=prompt, decoder_attention_mask=prompt.ne(0))
-                ids, _ = model_generate(model, tok2, dict(mk), dict(gk))
-                gen_out[f"{flavour}/{cname}/ids"] = ids.numpy()
+        gen_out.update(long_context_golden(model, tok2, cfg, flavour))
         ids, mask = cases.teacher_forcing_case(cfg)
         out = model(frames=cases.model_pcm(cfg, 2, 1), decoder_input_ids=ids, decoder_attention_mask=mask)
         gen_out[f"{flavour}/teacher_logits"] = out.logits.float().numpy()[:, ::3, ::37]
@@ -153,8 +149,20 @@ def main():
                                     np.log(diff.betas), diff.posterior_mean_coef1, diff.posterior_mean_coef2], 1)
     np.savez_compressed(os.path.join(OUT, "dit_reference.npz"), **dit_out, **{f"meta_{k}": v for k, v in meta.items()})
     make_slider_golden(meta)
+    make_pin_golden(meta)
     for f in sorted(os.listdir(OUT)):
         print(f, os.path.getsize(os.path.join(OUT, f)))
+
+
+def long_context_golden(model, tok, cfg, flavour):
+    """Prompts of 150 and 600 tokens (left-padded batch of 2) through the reference model_generate: {flavour/case/ids: ids}."""
+    from osuT5.osuT5.inference.server import model_generate
+    out = {}
+    for cname, (prompt, gk, seed) in cases.long_context_cases().items():
+        mk = dict(inputs=cases.model_pcm(cfg, prompt.shape[0], seed), decoder_input_ids=prompt, decoder_attention_mask=prompt.ne(0))
+        ids, _ = model_generate(model, tok, dict(mk), dict(gk))
+        out[f"{flavour}/{cname}/ids"] = ids.numpy()
+    return out
 
 
 def make_slider_golden(meta=None):
@@ -184,6 +192,124 @@ def make_slider_golden(meta=None):
     np.savez_compressed(os.path.join(OUT, "slider_reference.npz"), types=np.array(types, dtype=np.int32), offsets=np.array(offs, dtype=np.int32),
                         points=np.concatenate(pts).astype(np.float32), lengths=np.array(lens, dtype=np.float32), max_length=np.array(maxl),
                         end_pos=np.stack(ends), **({f"meta_{k}": v for k, v in (meta or {}).items()}))
+
+
+def slider_class_cases():
+    """Seeded random sliders of every curve type (with red anchors): (type, control points, length)."""
+    rng = np.random.default_rng(7)
+    out = []
+    for typ in ("Bezier", "PerfectCurve", "Catmull", "Linear"):
+        for k in range(60):
+            ncp = int(rng.integers(2, 10)) if typ != "PerfectCurve" else int(rng.choice([3, 3, 4, 2]))
+            cps = (rng.random((ncp, 2)) * np.array([512, 384])).astype(np.float32)
+            if ncp >= 4 and k % 4 == 0:
+                j = int(rng.integers(1, ncp - 2)); cps[j + 1] = cps[j]
+            out.append((typ, cps, float(rng.random() * 500 + 5)))
+    return out
+
+
+def v29_pin_config():
+    import dataclasses
+    from mapperatorinator_b200 import v29_model_config
+    return dataclasses.replace(v29_model_config(), mel=MelConfig("torchaudio", n_mels=80))
+
+
+def v29_bench_window_case(cfg):
+    """The bench workload's second window (50-token prompt, look-back + look-ahead processors, min_new_tokens), 10 greedy tokens."""
+    import bench
+    g = torch.Generator().manual_seed(0)
+    pcm = torch.randn(1, cfg.samples_per_window, generator=g) * 0.1
+    prompt = torch.tensor([bench.prompt_for(1, [list(range(100, 164))])])
+    P = prompt.shape[1]
+    gk = bench.gen_kwargs(1, 211, P)
+    gk.update(max_length=P + 10, min_new_tokens=10, precision="fp32")
+    return dict(inputs=pcm, decoder_input_ids=prompt, decoder_attention_mask=prompt.ne(0)), gk
+
+
+def v29_logits_case(cfg):
+    g = torch.Generator().manual_seed(0)
+    pcm = torch.randn(1, cfg.samples_per_window, generator=g) * 0.1
+    ids = torch.randint(17, cfg.vocab_size_in, (1, 12), generator=g)
+    return pcm, ids
+
+
+def timestep_case():
+    g = torch.Generator().manual_seed(4)
+    T = 37
+    seq_o = torch.rand(T, generator=g) * 180000.0
+    seq_d = torch.rand(T, generator=g) * 400.0
+    types = torch.randint(0, 16, (T,), generator=g)
+    return seq_o, seq_d, types
+
+
+def trim_reference(layout, cases_):
+    """The reference's own `Processor.add_predicted_tokens_to_context` (processor.py:1022-1052) run on a stand-in `self` that records
+    what reaches `_decode`: one token list per (types_first, case)."""
+    import types
+    from oracle import ref_import
+    ref_import.install_stubs()
+    from osuT5.osuT5.inference import processor as rp
+    from osuT5.osuT5.tokenizer import ContextType
+    seen = []
+    fake = types.SimpleNamespace(
+        tokenizer=types.SimpleNamespace(eos_id=layout.eos_id, context_eos={ContextType(k): v for k, v in layout.context_eos.items()}),
+        lookback_time_range=range(layout.time_shift_start, layout.lookback_end(4092.0)),                 # processor.py:85
+        lookahead_time_range=range(layout.lookback_end(4910.4), layout.time_shift_end),                  # processor.py:88
+        types_first=True, eos_time=0.0, lookahead_max_time=4910.4,
+        _decode=lambda toks, frame_time: seen.append(list(toks)) or [], _trim_events_after_time=lambda *a: None)
+    old = rp.update_event_times
+    rp.update_event_times = lambda *a, **k: None
+    out = []
+    try:
+        for types_first in (True, False):
+            fake.types_first = types_first
+            for toks, tlb, tla in cases_:
+                seen.clear()
+                ctx = {"context_type": ContextType("map"), "events": [], "event_times": []}
+                rp.Processor.add_predicted_tokens_to_context(fake, ctx, torch.tensor(toks, dtype=torch.long).tolist(), 1234.0, tlb, tla)
+                out.append(seen[0])
+    finally:
+        rp.update_event_times = old
+    return out
+
+
+def make_pin_golden(meta=None):
+    """tests/golden/reference_pins.npz: outputs of the reference's own functions that the oracle is pinned against — slider end points
+    (SliderPath), token trimming (Processor.add_predicted_tokens_to_context), osu_diffusion.timestep_embedding, one teacher-forced
+    pass and 10 greedy ids at full whisper-small dimensions (Mapperatorinator.forward, server.model_generate)."""
+    from oracle import ref_import
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from test_host_logic import _trim_cases
+    out = {}
+    SP = ref_import.reference_slider_path()
+    ends, mls = [], []
+    for typ, cps, length in slider_class_cases():
+        sp = SP(typ, cps)
+        ml = float(sp.get_distance())
+        mls.append(ml)
+        ends.append(np.asarray(sp.position_at(length / ml), dtype=np.float64) if ml != 0 else np.full(2, np.nan))
+    out["slider/max_length"] = np.array(mls)
+    out["slider/end_pos"] = np.stack(ends)
+    layout = TokenLayout.from_json(os.path.join(OUT, "tokenizer_v29.json"))
+    trims = trim_reference(layout, _trim_cases(layout))
+    out["trim/offsets"] = np.cumsum([0] + [len(t) for t in trims]).astype(np.int64)
+    out["trim/tokens"] = np.array(sum(trims, []), dtype=np.int64)
+    ref_import.install_stubs()
+    from osu_diffusion import timestep_embedding as ref_te
+    seq_o, seq_d, _ = timestep_case()
+    out["timestep/time"] = ref_te(seq_o * 0.1, 128).numpy()
+    out["timestep/distance"] = ref_te(seq_d, 128).numpy()
+    cfg = v29_pin_config()
+    model, tok, _ = ref_build.reference_model(cfg, mel_impl="torchaudio")
+    sd = init_model_state_dict(cfg, 0)
+    ref_build.load_state_dict_into_reference(model, sd)
+    pcm, ids = v29_logits_case(cfg)
+    with torch.no_grad():
+        out["v29/logits"] = model(frames=pcm, decoder_input_ids=ids, decoder_attention_mask=ids.ne(0)).logits.float().numpy()
+        from osuT5.osuT5.inference.server import model_generate
+        mk, gk = v29_bench_window_case(cfg)
+        out["v29/greedy_ids"] = model_generate(model, tok, dict(mk), dict(gk))[0].numpy()
+    np.savez_compressed(os.path.join(OUT, "reference_pins.npz"), **out, **{f"meta_{k}": v for k, v in (meta or {}).items()})
 
 
 if __name__ == "__main__":

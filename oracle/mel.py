@@ -4,11 +4,11 @@ TEST INFRASTRUCTURE (see oracle/__init__.py).
 
 * `nnaudio_*`  — v29 (`configs/model/default.yaml:29-38`): nnAudio==0.3.4 `features.MelSpectrogram(sr, n_fft, n_mels,
   hop_length, center=True, fmin, fmax, pad_mode)` with its defaults `window='hann', power=2.0, htk=False, norm=1`.
-  nnAudio is a third-party dependency (requirements.txt:3) that is NOT installed here and NOT in /root/reference:
+  nnAudio is a third-party dependency (requirements.txt:3) that is NOT installed and NOT vendored in the original project:
   this restates its published algorithm — conv1d STFT with `cos/sin(2*pi*k*n/n_fft) * hann[n]` kernels, magnitude
   `sqrt(re^2 + im^2)`, `** power`, `mel_basis @ spec` with the librosa Slaney filterbank.  **parity unpinned** vs nnAudio.
-* `torchaudio_*` — v30+ (`spectrogram.py:38-49`): restated AND pinned against the installed torchaudio in
-  tests/test_oracle_vs_reference.py.
+* `torchaudio_*` — v30+ (`spectrogram.py:38-49`): restated AND pinned against the installed torchaudio through
+  tests/golden/mel_reference.npz.
 Output layout follows spectrogram.py:79-83: optional log1p, then permute to (B, frames, n_mels).
 """
 from __future__ import annotations

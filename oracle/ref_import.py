@@ -1,7 +1,8 @@
-"""Import the UNMODIFIED reference classes from /root/reference (build container only).
+"""Import the UNMODIFIED reference classes from a checkout of the original Mapperatorinator project, located by the
+MAPPERATORINATOR_REFERENCE environment variable.
 
-TEST INFRASTRUCTURE. Used only by `oracle/make_golden.py` (fixture generation) and by
-`tests/test_oracle_vs_reference.py` (skipped when /root/reference is absent, i.e. on the GPU box).
+TEST INFRASTRUCTURE. Used only by `oracle/make_golden.py` (fixture generation); the tests compare against the fixtures it
+stores under tests/golden.
 Follows the stub recipe of SURVEY.md §8(c): third-party modules that are not installed here
 (hydra, omegaconf, slider, pydub, peft, accelerate, ...) are replaced by MagicMock modules so that
 the reference's own numerics (Mapperatorinator, model_generate, DiT, create_diffusion) import unmodified.
@@ -14,7 +15,7 @@ import sys
 import types
 from unittest.mock import MagicMock
 
-REFERENCE_ROOT = os.environ.get("MAPPERATORINATOR_REFERENCE", "/root/reference")
+REFERENCE_ROOT = os.environ.get("MAPPERATORINATOR_REFERENCE", "")
 
 _STUBS = [
     "slider", "slider.beatmap", "slider.mod", "slider.curve", "slider.position", "pydub",
@@ -25,7 +26,7 @@ _STUBS = [
 
 
 def reference_available() -> bool:
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "osuT5"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "osuT5"))
 
 
 def install_stubs() -> None:

@@ -32,10 +32,10 @@ def test_gemm_epilogues(M, N, K, act):
 
 @pytest.mark.parametrize("M,N,K", [(1024, 768, 768), (640, 3072, 388), (512, 130, 3072), (2048, 2304, 768), (1500, 768, 2304)])
 def test_gemm_tcgen05_3xtf32_matches_fp64(M, N, K):
-    """The tensor-core path must be fp32-grade (3xTF32 split, fp32 TMEM accumulation): error vs an fp64 product far below plain
-    TF32 (~1e-3).  Measured on B200: the operand split is exact to ~2^-22 but the tensor core's fp32 accumulator truncates (not
-    rounds) each partial sum, so the error grows with K to ~8e-6 relative at K = 3072 (SIMT FMA kernel: ~1e-6).  The bound below
-    is that measured envelope with 2.5x head-room; token-level parity with tensor cores on is covered in test_gpu_model."""
+    """The tensor-core path must be fp32-grade (3xTF32 split, fp32 accumulation): error vs an fp64 product far below plain
+    TF32 (~1e-3).  The operand split is exact to ~2^-22 but the tensor core's fp32 accumulator truncates (not rounds) each
+    partial sum, so the error grows with K (to ~8e-6 relative at K = 3072; SIMT FMA kernel: ~1e-6).  The bound below leaves
+    head-room over that envelope; token-level parity with tensor cores on is covered in test_gpu_model."""
     from mapperatorinator_b200 import ops
     g = _g(M + N + K)
     a, w = torch.randn(M, K, generator=g), torch.randn(N, K, generator=g) / math.sqrt(K)
@@ -107,7 +107,7 @@ def test_attention_masks(Tq, Tk, mode):
 @pytest.mark.parametrize("Tq,Tk,mode,scale", [(1024, 1024, "band", 0.125), (512, 512, "none", 1.0), (130, 700, "none", 0.3),
                                               (333, 333, "causal", 1.0), (260, 260, "band", 1.0)])
 def test_attention_tensor_cores(Tq, Tk, mode, scale):
-    """tcgen05 flash attention (3xTF32 for Q.K^T and P.V, softmax state in the row's own thread) vs an fp64 reference, and against the
+    """wgmma flash attention (3xTF32 for Q.K^T and P.V, online softmax in registers) vs an fp64 reference, and against the
     fp32 SIMT kernel it replaces: DiT shape (T = 1024, +-128 band), encoder shape (T = 512), ragged tiles, causal with left padding."""
     from mapperatorinator_b200 import _lib, ops
     lib = _lib.load()

@@ -94,8 +94,6 @@ def test_greedy_generate_long_context(tiny, layout, gen_gold, case, path):
     from mapperatorinator_b200.server import model_generate
     from oracle import generate as go
     flavour, cfg, sd, model = tiny
-    if flavour != "torchaudio":
-        pytest.skip("one mel flavour is enough for the decoder-side path")
     prompt, gk, seed = cases.long_context_cases()[case]
     mk = dict(inputs=cases.model_pcm(cfg, 2, seed), decoder_input_ids=prompt, decoder_attention_mask=prompt.ne(0))
     want, _ = go.model_generate(sd, cfg, layout, dict(mk), dict(gk))

@@ -1,5 +1,5 @@
 """The CPU oracle against the committed reference outputs (tests/golden/*.npz, produced by oracle/make_golden.py from the
-UNMODIFIED reference classes).  Runs anywhere: no GPU, no /root/reference."""
+UNMODIFIED reference classes).  Runs anywhere: no GPU, no reference checkout."""
 import os
 
 import numpy as np

@@ -1,62 +1,44 @@
-"""Live pin of the oracle against the UNMODIFIED reference classes (build container only: skipped when /root/reference
-is absent, e.g. on the GPU box — there the committed tests/golden fixtures carry the same pin)."""
+"""The oracle against outputs of the UNMODIFIED reference classes at full whisper-small dimensions and in the diffusion host helpers,
+stored in tests/golden/reference_pins.npz by oracle/make_golden.py (make_pin_golden).  Runs anywhere: no GPU, no reference checkout."""
+import os
+
 import numpy as np
 import pytest
 import torch
 
-from oracle import ref_import
+from oracle import make_golden
 
-pytestmark = [pytest.mark.reference, pytest.mark.skipif(not ref_import.reference_available(), reason="/root/reference not present")]
-
-
-def test_golden_fixtures_are_reproducible(tmp_path, monkeypatch):
-    """Re-running oracle/make_golden.py reproduces the committed fixtures bit-for-bit (same image, same seeds)."""
-    import os
-    from oracle import make_golden
-    gold_dir = make_golden.OUT
-    monkeypatch.setattr(make_golden, "OUT", str(tmp_path))
-    make_golden.main()
-    for f in ("generate_reference.npz", "dit_reference.npz", "mel_reference.npz", "processors_reference.npz"):
-        a, b = np.load(os.path.join(gold_dir, f)), np.load(os.path.join(str(tmp_path), f))
-        assert sorted(a.files) == sorted(b.files)
-        for k in a.files:
-            assert np.array_equal(a[k], b[k]), (f, k)
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
-def test_v29_dims_single_step_logits():
+@pytest.fixture(scope="module")
+def pins():
+    return np.load(os.path.join(GOLDEN, "reference_pins.npz"))
+
+
+def test_v29_dims_single_step_logits(pins):
     """One teacher-forced pass at full whisper-small dimensions: reference `Mapperatorinator.forward` vs the oracle."""
-    from mapperatorinator_b200 import MelConfig, v29_model_config
     from mapperatorinator_b200.weights import init_model_state_dict
-    from oracle import ref_build, whisper as wo
-    import dataclasses
-    cfg = dataclasses.replace(v29_model_config(), mel=MelConfig("torchaudio", n_mels=80))
-    model, tok, _ = ref_build.reference_model(cfg, mel_impl="torchaudio")
+    from oracle import whisper as wo
+    cfg = make_golden.v29_pin_config()
     sd = init_model_state_dict(cfg, 0)
-    ref_build.load_state_dict_into_reference(model, sd)
-    g = torch.Generator().manual_seed(0)
-    pcm = torch.randn(1, cfg.samples_per_window, generator=g) * 0.1
-    ids = torch.randint(17, cfg.vocab_size_in, (1, 12), generator=g)
+    pcm, ids = make_golden.v29_logits_case(cfg)
+    ref = torch.from_numpy(pins["v29/logits"])
     with torch.no_grad():
-        ref = model(frames=pcm, decoder_input_ids=ids, decoder_attention_mask=ids.ne(0)).logits.float()
         out = wo.forward_logits(sd, cfg, pcm, ids, ids.ne(0))
     assert torch.allclose(out, ref, rtol=1e-3, atol=1e-3), (out - ref).abs().max()
     assert torch.equal(out.argmax(-1), ref.argmax(-1))
 
 
-def test_diffusion_host_helpers_match_reference():
+def test_diffusion_host_helpers_match_reference(pins):
     """`timestep_embedding`, the seq_c layout of `events_to_sequence` (diffusion_pipeline.py:380-387) and the band mask loop
     (:146-148) — the host-side tensor preparation around stage (iii) — against the reference's own functions."""
     from mapperatorinator_b200 import diffusion as md
-    ref_import.install_stubs()
-    from osu_diffusion import timestep_embedding as ref_te
-    g = torch.Generator().manual_seed(4)
-    T = 37
-    seq_o = torch.rand(T, generator=g) * 180000.0
-    seq_d = torch.rand(T, generator=g) * 400.0
-    types = torch.randint(0, 16, (T,), generator=g)
-    for v in (seq_o * 0.1, seq_d):
-        assert torch.equal(md.timestep_embedding(v, 128), ref_te(v, 128))
-    want = torch.cat([ref_te(seq_o * 0.1, 128).T, ref_te(seq_d, 128).T, torch.nn.functional.one_hot(types, 16).float().T], 0)
+    seq_o, seq_d, types = make_golden.timestep_case()
+    ref_time, ref_dist = torch.from_numpy(pins["timestep/time"]), torch.from_numpy(pins["timestep/distance"])
+    assert torch.equal(md.timestep_embedding(seq_o * 0.1, 128), ref_time)
+    assert torch.equal(md.timestep_embedding(seq_d, 128), ref_dist)
+    want = torch.cat([ref_time.T, ref_dist.T, torch.nn.functional.one_hot(types, 16).float().T], 0)
     assert torch.equal(md.build_context(seq_o, seq_d, types), want)
     # band mask: the reference fills it column by column (diffusion_pipeline.py:146-148)
     L, w = 50, 8
@@ -66,33 +48,17 @@ def test_diffusion_host_helpers_match_reference():
     assert torch.equal(md.band_attention_mask(L, w), ref_mask)
 
 
-def test_v29_dims_bench_window_greedy_ids():
+def test_v29_dims_bench_window_greedy_ids(pins, layout):
     """The bench workload's second window (50-token prompt, look-back + look-ahead processors, min_new_tokens) at FULL whisper-small
-    dimensions through the unmodified reference `server.model_generate`, against the oracle: 10 greedy tokens, ids bit-exact.
-    (The bench then asserts GPU ids == oracle ids on its CPU sample, closing the chain reference -> oracle -> engine at v29 dims.)"""
-    import dataclasses
-    import os
-    import sys
-    from mapperatorinator_b200 import MelConfig, TokenLayout, v29_model_config
+    dimensions: the ids of the unmodified reference `server.model_generate` against the oracle's, 10 greedy tokens, bit-exact.
+    (The bench then checks the GPU ids against the oracle over the song, closing the chain reference -> oracle -> engine at v29 dims.)"""
     from mapperatorinator_b200.weights import init_model_state_dict
-    from oracle import generate as go, ref_build
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    sys.path.insert(0, root)
-    import bench
-    cfg = dataclasses.replace(v29_model_config(), mel=MelConfig("torchaudio", n_mels=80))
-    model, tok, _ = ref_build.reference_model(cfg, mel_impl="torchaudio")          # installs the import stubs
-    from osuT5.osuT5.inference.server import model_generate
+    from oracle import generate as go
+    cfg = make_golden.v29_pin_config()
     sd = init_model_state_dict(cfg, 0)
-    ref_build.load_state_dict_into_reference(model, sd)
-    layout = TokenLayout.from_tokenizer(tok)
-    g = torch.Generator().manual_seed(0)
-    pcm = torch.randn(1, cfg.samples_per_window, generator=g) * 0.1
-    prompt = torch.tensor([bench.prompt_for(1, [list(range(100, 164))])])
-    P = prompt.shape[1]
-    gk = bench.gen_kwargs(1, 211, P)
-    gk.update(max_length=P + 10, min_new_tokens=10, precision="fp32")
-    mk = dict(inputs=pcm, decoder_input_ids=prompt, decoder_attention_mask=prompt.ne(0))
+    mk, gk = make_golden.v29_bench_window_case(cfg)
+    P = mk["decoder_input_ids"].shape[1]
+    ref_ids = torch.from_numpy(pins["v29/greedy_ids"])
     with torch.no_grad():
-        ref_ids, _ = model_generate(model, tok, dict(mk), dict(gk))
         ora_ids, _ = go.model_generate(sd, cfg, layout, dict(mk), dict(gk))
     assert torch.equal(ref_ids, ora_ids), (ref_ids[0, P:].tolist(), ora_ids[0, P:].tolist())

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Dense attention, tensor-core (tcgen05 3xTF32, attention_tc.cu) vs fp32 SIMT (attention.cu), CUDA-event timed through the C ABI.
+"""Dense attention, tensor-core (wgmma 3xTF32, attention_tc.cu) vs fp32 SIMT (attention.cu), CUDA-event timed through the C ABI.
 Shapes: Whisper encoder self-attention of a 16-window chunk (B = 16, H = 12, T = 512) and the DiT block (B = 2, H = 12, T = 1024, +-128 band)."""
 import os
 import sys
@@ -31,5 +31,5 @@ for name, B, H, T, mode, band in (("encoder 16 windows", 16, 12, 512, "none", 0)
         res[tc] = (e0.elapsed_time(e1) / 20.0, out)
     _lib.check(lib.mb200_set_attention_tc(1, 256))
     err = (res[0][1] - res[1][1]).abs().max().item()
-    print(f"{name:24s} SIMT {res[0][0] * 1e3:8.1f} us   tcgen05 (prep + kernel) {res[1][0] * 1e3:8.1f} us   "
+    print(f"{name:24s} SIMT {res[0][0] * 1e3:8.1f} us   wgmma (prep + kernel) {res[1][0] * 1e3:8.1f} us   "
           f"{flops / res[1][0] / 1e9:6.1f} TFLOP/s algorithmic   max |diff| {err:.2e}")

@@ -1,7 +1,7 @@
 // Micro-benchmark behind the megakernel's phase design (DESIGN.md 4.1): what does one "everybody reads the activation vector
-// right after a grid barrier" round trip cost on B200, and why?
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o l2_hotspot_bench tools/l2_hotspot_bench.cu && ./l2_hotspot_bench
-// One persistent cooperative grid (148 CTAs x 512 threads).  Every iteration: producers write their slice of a 768-float vector,
+// right after a grid barrier" round trip cost, and why?
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o l2_hotspot_bench tools/l2_hotspot_bench.cu && ./l2_hotspot_bench
+// One persistent cooperative grid (one CTA per SM x 512 threads).  Every iteration: producers write their slice of a 768-float vector,
 // grid barrier (release add + acquire poll, as in decode_mega.cu), then warp 0 of every CTA loads the whole vector with ld.global.cg
 // and we time issue -> data usable with clock64.  Modes:
 //   0  all CTAs read the SAME freshly written vector                       (what LayerNorm staging does)
