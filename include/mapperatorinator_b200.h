@@ -106,6 +106,20 @@ int mb200_model_generate(mb200_model* m, const int32_t* slots, int32_t batch, co
                          int32_t prompt_len, const int64_t* neg_prompt, const uint8_t* neg_mask, const uint8_t* vflags,
                          const mb200_generate_params* params, int64_t* out_ids, int32_t* out_len, void* cuda_stream);
 
+/* The same call with HF beam search (generate(num_beams=K, do_sample=False), length_penalty 1.0, early_stopping False), 2 <= K <= 4:
+ * the engine runs batch * K decoder rows (2x under classifier-free guidance; max_batch must cover them).  Same inputs as
+ * mb200_model_generate plus
+ *   num_beams                     K
+ *   fill_id                       the id written past a shorter hypothesis (HF: pad_token_id, or the first EOS id when that is 0)
+ * and returns the best finished hypothesis of every item:
+ *   out_ids[batch, out_len]       int64, prompt + generated, out_len = prompt_len + the longest generated length in the batch
+ *   out_scores[batch]             its score (sum of processed log-probs / generated length), HF's sequences_scores
+ */
+int mb200_model_generate_beams(mb200_model* m, const int32_t* slots, int32_t batch, const int64_t* prompt, const uint8_t* prompt_mask,
+                               int32_t prompt_len, const int64_t* neg_prompt, const uint8_t* neg_mask, const uint8_t* vflags,
+                               const mb200_generate_params* params, int32_t num_beams, int64_t fill_id, int64_t* out_ids,
+                               int32_t* out_len, float* out_scores, void* cuda_stream);
+
 /* Mapperatorinator.forward teacher-forced logits (server.model_forward, server.py:159-181), no CFG mixing.
  * ids: HOST int64 [batch, len]; mask HOST uint8; logits_out: DEVICE f32 [batch, len, vocab_size_out]. */
 int mb200_model_forward_logits(mb200_model* m, const int32_t* slots, int32_t batch, const int64_t* ids, const uint8_t* mask,
@@ -174,6 +188,16 @@ int mb200_model_set_option(mb200_model* m, const char* name, int32_t value);
 int mb200_model_logits_chain(mb200_model* m, const float* logits, int32_t B, int32_t use_cfg, const int64_t* ids, int32_t L, int32_t prompt_len,
                              const uint8_t* vflags, const mb200_generate_params* gp, int32_t step, int32_t has_last_scores, float* scores_out,
                              int64_t* chosen_out, void* cuda_stream);
+/* Parity hook for beam search: ONE selection step of the beam kernels on caller-supplied logits, from an empty finished store.
+ * logits DEVICE [rows, V] (rows = 2*B*K under CFG, negative-prompt rows first); ids HOST [B*K, L] running sequences; run_scores HOST [B*K].
+ * logprobs_out DEVICE [B*K, V] processed log-probs; HOST [B*K]: top_out first K candidates per item (flat index beam * V + token),
+ * parent_out batch row each new running beam continues, token_out / score_out its token and running score, fin_score_out /
+ * fin_len_out / fin_flag_out the finished store (-1e9 / 0 / 0 where empty); fin_ids_out HOST [B*K, L + 1]. */
+int mb200_model_beam_step(mb200_model* m, const float* logits, int32_t B, int32_t num_beams, int32_t use_cfg, const int64_t* ids, int32_t L,
+                          int32_t prompt_len, const uint8_t* vflags, const mb200_generate_params* gp, const float* run_scores, int32_t step,
+                          int32_t has_last_scores, float* logprobs_out, int32_t* top_out, int32_t* parent_out, int64_t* token_out,
+                          float* score_out, float* fin_score_out, int32_t* fin_len_out, uint8_t* fin_flag_out, int64_t* fin_ids_out,
+                          void* cuda_stream);
 /* option "graph": 1 (default) = every step of mb200_dit_sample_loop is one replay of a captured CUDA graph, 0 = eager launches. */
 int mb200_dit_set_option(mb200_dit* d, const char* name, int32_t value);
 /* Re-runs the token step eagerly `iters` times on the state of the last generate() call with CUDA events around every

@@ -35,7 +35,7 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(GemvParams p) {
     }
 }
 
-template <int KMAX>
+template <int KMAX, bool TABLE = false>
 __global__ void __launch_bounds__(128, KMAX == 64 ? 6 : 4) decode_attention_kernel(DecAttnParams p) {
     __shared__ float sc[128];
     __shared__ float red[4][64];
@@ -47,8 +47,8 @@ __global__ void __launch_bounds__(128, KMAX == 64 ? 6 : 4) decode_attention_kern
     const int r = blockIdx.z;
     const int slot = p.row_slot ? p.row_slot[r] : r;
     AttnRegs<4, KMAX> regs;
-    decode_attention_load<4, KMAX>(p, blockIdx.x, blockIdx.y, r, slot, L, P, threadIdx.x, regs);
-    decode_attention_body<4, KMAX>(p, blockIdx.x, blockIdx.y, r, slot, L, P, sc, red, stat, threadIdx.x, regs);
+    decode_attention_load<4, KMAX, TABLE>(p, blockIdx.x, blockIdx.y, r, slot, L, P, threadIdx.x, regs);
+    decode_attention_body<4, KMAX, TABLE>(p, blockIdx.x, blockIdx.y, r, slot, L, P, sc, red, stat, threadIdx.x, regs);
 }
 
 // batch form: one warp per (split, head, row) unit, 8 units per CTA (see decode_attention_warp_body)
@@ -157,6 +157,10 @@ int launch_decode_attention(const DecAttnParams& p, cudaStream_t stream, bool pd
     // one-warp-per-unit form for rows > 2 — the same arithmetic value for value (parity-tested), kept as the starting point for a
     // persistent multi-unit kernel.
     static const int batch_form = [] { const char* e = getenv("MB200_ATTN_BATCH"); return e ? atoi(e) : 0; }();
+    if (p.kv_src) {        // beam search: self attention through the source-row table
+        if (p.chunk <= 64) return launch_with_attrs(decode_attention_kernel<64, true>, dim3(p.n_splits, p.H, p.rows), dim3(128), 0, stream, pdl, p);
+        return launch_with_attrs(decode_attention_kernel<128, true>, dim3(p.n_splits, p.H, p.rows), dim3(128), 0, stream, pdl, p);
+    }
     if (p.rows > 2 && batch_form) {
         const int units = p.rows * p.H * p.n_splits;
         return launch_with_attrs(decode_attention_warp_kernel, dim3((units + 7) / 8), dim3(256), 0, stream, pdl, p);

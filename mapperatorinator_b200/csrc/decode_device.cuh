@@ -306,6 +306,11 @@ __device__ __forceinline__ void decode_attention_merge(const DecAttnParams& p, i
 // ---------------------------------------------------------------------------------------------------------------------
 // split-KV decode attention for one (split s, head h, row r); NW warps cooperate; smem: sc[128], red[NW][64], stat[2]
 // ---------------------------------------------------------------------------------------------------------------------
+// cache address of key position t of decoder row r, head h, through the source-row table
+__device__ __forceinline__ const float* table_row(const DecAttnParams& p, int r, int t, int h, const float* base) {
+    return base + (long long)__ldcg(p.kv_src + (long long)r * p.kv_src_ld + t) * p.row_stride + h * 64 + (long long)t * p.tok_stride;
+}
+
 // K / validity / V operands of one (split, head, row) unit, held in registers between the load and the compute half so that the load
 // can be issued EARLY: cross-attention K/V are constants of the call, the megakernel requests them before the preceding grid barrier.
 // KMAX = keys a unit may hold: 128 (default), or 64 for launches whose chunks are 64 keys (the batched per-phase kernel: half the K
@@ -318,7 +323,9 @@ struct AttnRegs {
     float2 vpre[PV_PRE];
 };
 
-template <int NW, int KMAX = 128>
+// TABLE: self-attention keys are read through the per-position source-row table p.kv_src (beam search: key t of row r lives in
+// cache row kv_src[r][t]); the arithmetic is unchanged.
+template <int NW, int KMAX = 128, bool TABLE = false>
 __device__ __forceinline__ void decode_attention_load(const DecAttnParams& p, int s, int h, int r, int slot, int L, int P, int tid, AttnRegs<NW, KMAX>& R) {
     constexpr int SC_ITERS = AttnRegs<NW, KMAX>::SC_ITERS, PV_PRE = AttnRegs<NW, KMAX>::PV_PRE;
     const int lane = tid & 31, warp = tid >> 5;
@@ -336,7 +343,7 @@ __device__ __forceinline__ void decode_attention_load(const DecAttnParams& p, in
         const int kk = it * 4 * NW + warp * 4 + kq;
         R.kvalid[it] = 1;
         if (kk < nk) {
-            const float* kr = kb + kk * tok + sub * 8;
+            const float* kr = (TABLE ? table_row(p, r, k_begin + kk, h, p.kc) : kb + kk * tok) + sub * 8;
             R.ka[it] = ldcg4(kr); R.kb4[it] = ldcg4(kr + 4);
             if (kv && kk < n_prompt) R.kvalid[it] = kv[kk];
         } else {
@@ -349,12 +356,12 @@ __device__ __forceinline__ void decode_attention_load(const DecAttnParams& p, in
 #pragma unroll
         for (int i = 0; i < PV_PRE; ++i) {
             const int kk = warp + 4 * i;
-            R.vpre[i] = kk < nk ? ldcg2(vb + kk * tok + lane * 2) : make_float2(0.f, 0.f);
+            R.vpre[i] = kk < nk ? ldcg2((TABLE ? table_row(p, r, k_begin + kk, h, p.vc) : vb + kk * tok) + lane * 2) : make_float2(0.f, 0.f);
         }
     }
 }
 
-template <int NW, int KMAX = 128>
+template <int NW, int KMAX = 128, bool TABLE = false>
 __device__ __forceinline__ void decode_attention_body(const DecAttnParams& p, int s, int h, int r, int slot, int L, int P, float* sc,
                                                       float (*red)[64], float* stat, int tid, const AttnRegs<NW, KMAX>& R,
                                                       unsigned long long* dbg = nullptr) {
@@ -429,7 +436,7 @@ __device__ __forceinline__ void decode_attention_body(const DecAttnParams& p, in
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
                     const int kk = 32 * t + warp + 4 * i;
-                    vv[i] = kk < nk ? ldcg2(vb + kk * tok + lane * 2) : make_float2(0.f, 0.f);
+                    vv[i] = kk < nk ? ldcg2((TABLE ? table_row(p, r, k_begin + kk, h, p.vc) : vb + kk * tok) + lane * 2) : make_float2(0.f, 0.f);
                 }
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
@@ -870,33 +877,18 @@ static __device__ __forceinline__ int sample_greedy_regs(const SampleParams& p, 
     return bi == 0x7fffffff ? 0 : bi;
 }
 
-// The whole logits-processor chain + token selection + append for batch row b (one CTA of NT threads).
-// Deliberately NOT inlined and with rolled vocabulary loops: it runs once per token on one CTA; inlined and unrolled it was 70 KB of
-// the megakernel's 130 KB of code.  (A cold/warm re-run experiment later showed the per-layer phases are NOT instruction-fetch bound,
-// so this is about code size and register pressure of the caller, not about the 32 KB L1.5 instruction cache.)
-// Returns after the "last CTA" bookkeeping; the caller decides how the grid synchronises afterwards.
-// NT = threads of the calling CTA (512 in the per-phase kernel and the barrier megakernel, 256 in the dataflow megakernel).
+// The logits-processor chain of one batch row b (steps 0-5: min_new_tokens EOS mask, CFG, MonotonicTimeShift, TimeshiftBias,
+// temperature decided on row 0, LookbackBias) from p.logits into sm.s.  Shared by the token selection below (on logits) and by the
+// beam-search scores phase (beam.cu, on log-probs).
 template <int NT>
-static __device__ __noinline__ void sample_body(const SampleParams& p, int b, SampleSmem& sm) {
+static __device__ __forceinline__ void logits_chain(const SampleParams& p, int b, SampleSmem& sm, int L, int st_step, int st_has_last,
+                                                    bool suppress_eos) {
     float* s = sm.s;
-    int* sidx = sm.sidx;
     float* scratch = sm.scratch;
     const int tid = threadIdx.x;
     const SampleConfig& c = *p.cfg;
-    GenState* st = p.st;
     const int V = c.V, B = c.B;
-    const int L = ld_state(&st->cur_len);
-    const int st_prompt_len = ld_state(&st->prompt_len), st_min_new = ld_state(&st->min_new_tokens);
-    const int st_step = ld_state(&st->step), st_has_last = ld_state(&st->has_last_scores), st_max_length = ld_state(&st->max_length);
     long long* ids_row = p.ids + (long long)b * c.ids_ld;
-    const bool suppress_eos = st_min_new > 0 && (L - st_prompt_len) < st_min_new;
-
-    if (p.trace && tid == 0) p.trace[6] = (unsigned long long)clock64();
-    int chosen = 0;
-    const bool fast_greedy = p.ll_logits != nullptr && !c.do_sample && p.dbg_scores == nullptr && V <= VMAX;
-    if (fast_greedy) {
-        chosen = sample_greedy_regs<NT>(p, b, sm, L, st_step, st_has_last, suppress_eos);
-    } else {
     // (0)+(1): min_new_tokens EOS suppression, then classifier-free guidance on raw logits
     if (p.ll_logits) {
         sample_poll_ll<NT>(p, b, s, suppress_eos);
@@ -981,6 +973,36 @@ static __device__ __noinline__ void sample_body(const SampleParams& p, int b, Sa
             __syncthreads();
         }
     }
+}
+
+// The whole logits-processor chain + token selection + append for batch row b (one CTA of NT threads).
+// Deliberately NOT inlined and with rolled vocabulary loops: it runs once per token on one CTA; inlined and unrolled it was 70 KB of
+// the megakernel's 130 KB of code.  (A cold/warm re-run experiment later showed the per-layer phases are NOT instruction-fetch bound,
+// so this is about code size and register pressure of the caller, not about the 32 KB L1.5 instruction cache.)
+// Returns after the "last CTA" bookkeeping; the caller decides how the grid synchronises afterwards.
+// NT = threads of the calling CTA (512 in the per-phase kernel and the barrier megakernel, 256 in the dataflow megakernel).
+template <int NT>
+static __device__ __noinline__ void sample_body(const SampleParams& p, int b, SampleSmem& sm) {
+    float* s = sm.s;
+    int* sidx = sm.sidx;
+    float* scratch = sm.scratch;
+    const int tid = threadIdx.x;
+    const SampleConfig& c = *p.cfg;
+    GenState* st = p.st;
+    const int V = c.V, B = c.B;
+    const int L = ld_state(&st->cur_len);
+    const int st_prompt_len = ld_state(&st->prompt_len), st_min_new = ld_state(&st->min_new_tokens);
+    const int st_step = ld_state(&st->step), st_has_last = ld_state(&st->has_last_scores), st_max_length = ld_state(&st->max_length);
+    long long* ids_row = p.ids + (long long)b * c.ids_ld;
+    const bool suppress_eos = st_min_new > 0 && (L - st_prompt_len) < st_min_new;
+
+    if (p.trace && tid == 0) p.trace[6] = (unsigned long long)clock64();
+    int chosen = 0;
+    const bool fast_greedy = p.ll_logits != nullptr && !c.do_sample && p.dbg_scores == nullptr && V <= VMAX;
+    if (fast_greedy) {
+        chosen = sample_greedy_regs<NT>(p, b, sm, L, st_step, st_has_last, suppress_eos);
+    } else {
+    logits_chain<NT>(p, b, sm, L, st_step, st_has_last, suppress_eos);
 
     // (6)-(7) selection
     if (!c.do_sample) {

@@ -67,8 +67,9 @@ struct mb200_model {
     int* h_flag = nullptr;              // pinned
     // graph keys carry B as well as rows: the captured sample kernel's grid is dim3(B), and a CFG call (B = 1, rows = 2) must
     // never replay the graph of a plain batch-2 call (B = 2, rows = 2)
-    std::map<std::tuple<int, int, int>, cudaGraphExec_t> graphs;
-    std::map<std::tuple<int, int, int>, long long> graph_nodes;   // (rows, B, n_splits_self) -> token-step graph
+    // ... and the beam count: a beam call ends its token step in the beam kernels and must never replay a greedy graph of equal rows
+    std::map<std::tuple<int, int, int, int>, cudaGraphExec_t> graphs;
+    std::map<std::tuple<int, int, int, int>, long long> graph_nodes;   // (rows, B, n_splits_self, num_beams) -> token-step graph
     bool use_pdl = false;
     cudaStream_t cap_stream = nullptr;
     std::map<std::tuple<int, int, int, int>, int> prefill_seen;                                   // (rows, B, P, position rule)
@@ -91,6 +92,9 @@ struct mb200_model {
     DevBuf w_pcm;                       // single-window encode: engine-owned copy of the window's PCM (the captured graph reads it)
     std::map<int, std::pair<cudaGraphExec_t, long long>> enc_graphs;   // slot -> captured single-window encode (the drop-in per-call pattern), node count
     std::map<int, int> enc_seen;
+    // beam search state (allocated at the first beam call for max_batch rows, then fixed: captured graphs hold the pointers)
+    DevBuf b_kvsrc, b_logprobs, b_cand, b_runscore, b_finids[2], b_finscore, b_finlen, b_finflag, b_unsat;
+    DevBuf b_dbg;                       // beam-step parity hook outputs
     AttnCtx attn;                       // tensor-core attention scratch of the encoder (head-major tf32 copies of q | k | v^T)
     GemmCtx gemm;                       // this engine's GEMM scratch: split-K planes, tf32 activation copies, weight mirrors, error flag
 
@@ -610,7 +614,7 @@ static int self_splits(int max_length) { return max_length <= 128 ? 1 : (max_len
 // Either launches the 98 micro-phases of one token on `st` (eager / graph capture), or — when `collect` is given — records
 // them as phase descriptors for the persistent megakernel.  One definition, so both paths run the same arithmetic.
 static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaStream_t st, bool pdl,
-                      std::vector<MegaPhase>* collect = nullptr) {
+                      std::vector<MegaPhase>* collect = nullptr, const BeamParams* beam = nullptr) {
     auto emit_gemv = [&](const GemvParams& g) -> int {
         if (!collect) return launch_gemv(g, st, pdl);
         MegaPhase ph{}; ph.kind = 0; ph.g = g; collect->push_back(ph);
@@ -652,6 +656,7 @@ static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaSt
             a.part_o = po; a.part_ml = pml; a.rows = rows; a.H = H; a.n_splits = n_splits_self;
             a.chunk = n_splits_self == 1 ? 128 : chunk;      // contexts up to 128 tokens: one split per head, no merge step
             a.out = attn; a.out_ld = d; a.ticket = ticket;
+            if (beam) { a.kv_src = beam->kv_src; a.kv_src_ld = beam->kv_src_ld; }
             MB_TRY(emit_attn(a));
         }
         {   // out_proj + residual (the heads were merged by the attention phase)
@@ -708,6 +713,7 @@ static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaSt
         }
         return 0;
     }
+    if (beam) return launch_beam_step(*beam, B, st);
     MB_TRY(launch_sample(sample_params(m, rows), B, st, pdl));
     return 0;
 }
@@ -977,7 +983,7 @@ extern "C" int mb200_model_generate(mb200_model* m, const int32_t* slots, int32_
         return 0;
     }
     // ---- token loop, graph path: one graph replay per token, flag polled every few tokens ----
-    auto key = std::make_tuple(rows, (int)B, n_splits_self);
+    auto key = std::make_tuple(rows, (int)B, n_splits_self, 1);
     auto it = m->graphs.find(key);
     if (it == m->graphs.end()) {
         // capture on an engine-owned stream (the caller's stream may be the legacy default stream, which cannot capture)
@@ -1017,6 +1023,176 @@ extern "C" int mb200_model_generate(mb200_model* m, const int32_t* slots, int32_
     MB_CUDA_CHECK(cudaMemcpy2DAsync(out_ids, (size_t)L * 8, m->g_ids.p, (size_t)ids_ld * 8, (size_t)L * 8, B, cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
     *out_len = L;
+    return 0;
+}
+
+// beam-search state for max_batch rows, allocated once: captured graphs hold the pointers
+static int ensure_beam_buffers(mb200_model* m) {
+    const size_t R = (size_t)m->max_rows, ld = (size_t)m->cfg.tgt_seq_len, V = (size_t)m->cfg.vocab_size_out;
+    MB_TRY(m->b_kvsrc.ensure(R * ld * sizeof(int)));
+    MB_TRY(m->b_logprobs.ensure(R * V * sizeof(float)));
+    MB_TRY(m->b_cand.ensure(R * V * sizeof(float)));
+    MB_TRY(m->b_runscore.ensure(R * sizeof(float)));
+    MB_TRY(m->b_finids[0].ensure(R * ld * 8)); MB_TRY(m->b_finids[1].ensure(R * ld * 8));
+    MB_TRY(m->b_finscore.ensure(R * sizeof(float))); MB_TRY(m->b_finlen.ensure(R * sizeof(int)));
+    MB_TRY(m->b_finflag.ensure(R)); MB_TRY(m->b_unsat.ensure(R));
+    return 0;
+}
+
+static BeamParams beam_params(mb200_model* m, int rows, int K) {
+    const int V = m->cfg.vocab_size_out;
+    BeamParams bp{};
+    bp.sample = sample_params(m, rows);
+    bp.sample.logits = m->b_logprobs.as<float>(); bp.sample.logits_ld = V;
+    bp.logits = m->d_logits.as<float>(); bp.logits_ld = V;
+    bp.logprobs = m->b_logprobs.as<float>(); bp.cand = m->b_cand.as<float>(); bp.run_score = m->b_runscore.as<float>();
+    bp.kv_src = m->b_kvsrc.as<int>(); bp.kv_src_ld = m->cfg.tgt_seq_len;
+    bp.fin_ids[0] = m->b_finids[0].as<long long>(); bp.fin_ids[1] = m->b_finids[1].as<long long>();
+    bp.fin_score = m->b_finscore.as<float>(); bp.fin_len = m->b_finlen.as<int>(); bp.fin_flag = m->b_finflag.as<unsigned char>();
+    bp.unsat = m->b_unsat.as<unsigned char>();
+    bp.K = K; bp.V = V; bp.ids_ld = m->cfg.tgt_seq_len;
+    return bp;
+}
+
+// =====================================================================================================================
+// Beam search (num_beams = K in [2, 4]): HF's repeat_interleave expansion to B*K rows (2*B*K under classifier-free guidance),
+// prefill, the first selection with running scores [0, -1e9, ...], then one CUDA-graph replay per token (per-phase kernels only;
+// the megakernels stay greedy / sampling).  The self-attention cache is never copied: each row reads its history through the
+// source-row table that the selection kernel gathers by parent.
+extern "C" int mb200_model_generate_beams(mb200_model* m, const int32_t* slots, int32_t B, const int64_t* prompt, const uint8_t* prompt_mask,
+                                          int32_t P, const int64_t* neg_prompt, const uint8_t* neg_mask, const uint8_t* vflags,
+                                          const mb200_generate_params* gp, int32_t num_beams, int64_t fill_id, int64_t* out_ids,
+                                          int32_t* out_len, float* out_scores, void* stream) {
+    MB_REQUIRE(m && m->finalized, "model not finalized");
+    MB_REQUIRE(slots && prompt && vflags && gp && out_ids && out_len && out_scores, "null argument");
+    const auto& c = m->cfg;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int K = num_beams;
+    MB_REQUIRE(K >= 2 && K <= 4, "num_beams must be in [2, 4]");
+    MB_REQUIRE(!gp->do_sample, "beam sampling (do_sample with num_beams > 1) is not supported");
+    const bool use_cfg = neg_prompt != nullptr;
+    const int BK = B * K, rows = use_cfg ? 2 * BK : BK;
+    MB_REQUIRE(B >= 1 && rows <= m->max_rows, "batch * num_beams (x2 under classifier-free guidance) exceeds max_batch");
+    MB_REQUIRE(P >= 1 && P < gp->max_length && gp->max_length <= c.tgt_seq_len, "need 1 <= prompt_len < max_length <= tgt_seq_len");
+    for (int b = 0; b < B; ++b) MB_REQUIRE(slots[b] >= 0 && slots[b] < c.max_windows, "encoder slot out of range");
+    const int d = c.d_model, V = c.vocab_size_out, ids_ld = c.tgt_seq_len;
+    MB_REQUIRE(beam_select_smem_bytes(K, V, ids_ld) <= 220 * 1024, "beam candidates do not fit shared memory");
+    MB_TRY(ensure_beam_buffers(m));
+
+    // ---- host staging: row r is beam (r mod B*K) % K of item (r mod B*K) / K; rows [0, B*K) carry the negative prompt under CFG ----
+    std::vector<long long> pre((size_t)rows * P), idsrow((size_t)BK * ids_ld, (long long)gp->pad_token_id);
+    std::vector<unsigned char> kv((size_t)rows * ids_ld, 1);
+    std::vector<int> leftpad(rows, 0), rowslot(rows), kvsrc((size_t)rows * ids_ld, 0);
+    for (int r = 0; r < rows; ++r) {
+        const int b = (r % BK) / K;
+        const bool neg_row = use_cfg && r < BK;
+        const int64_t* src = neg_row ? neg_prompt : prompt;
+        const uint8_t* msk = neg_row ? (neg_mask ? neg_mask : prompt_mask) : prompt_mask;
+        int npad = 0; bool seen = false;
+        for (int t = 0; t < P; ++t) {
+            long long tok = src[(size_t)b * P + t];
+            MB_REQUIRE(tok >= 0 && tok < c.vocab_size_in, "prompt token id out of range");
+            pre[(size_t)r * P + t] = tok;
+            unsigned char ok = msk ? (msk[(size_t)b * P + t] != 0) : 1;
+            kv[(size_t)r * ids_ld + t] = ok;
+            if (!ok && !seen) ++npad; else seen = true;
+            kvsrc[(size_t)r * ids_ld + t] = r;
+        }
+        leftpad[r] = npad;
+        rowslot[r] = slots[b];
+    }
+    for (int j = 0; j < BK; ++j)
+        for (int t = 0; t < P; ++t) idsrow[(size_t)j * ids_ld + t] = prompt[(size_t)(j / K) * P + t];
+    std::vector<float> runscore(BK), finscore(BK, -1.0e9f);
+    for (int j = 0; j < BK; ++j) runscore[j] = j % K == 0 ? 0.f : -1.0e9f;
+    GenState gs{};
+    gs.cur_len = P; gs.prompt_len = P; gs.max_length = gp->max_length; gs.min_new_tokens = gp->min_new_tokens;
+    const SampleConfig sc = make_sample_config(gp, BK, use_cfg, V, ids_ld);
+
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_prefill_ids.p, pre.data(), pre.size() * 8, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_ids.p, idsrow.data(), idsrow.size() * 8, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_keyvalid.p, kv.data(), kv.size(), cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_leftpad.p, leftpad.data(), rows * 4, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_rowslot.p, rowslot.data(), rows * 4, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_vflags.p, vflags, c.vocab_size_in, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_state.p, &gs, sizeof(gs), cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_cfg.p, &sc, sizeof(sc), cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->b_kvsrc.p, kvsrc.data(), kvsrc.size() * 4, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->b_runscore.p, runscore.data(), BK * 4, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->b_finscore.p, finscore.data(), BK * 4, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->b_finlen.p, 0, BK * sizeof(int), st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->b_finflag.p, 0, BK, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->b_unsat.p, 1, B, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->d_ticket.p, 0, (size_t)m->max_rows * m->cfg.heads * sizeof(int), st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));   // host vectors go out of scope; the copies above are from pageable memory
+
+    const BeamParams bp = beam_params(m, rows, K);
+
+    MB_TRY(launch_prompt_scan(m->g_ids.as<long long>(), ids_ld, BK, P, m->g_vflags.as<unsigned char>(), sc.ts_start, sc.ts_end,
+                              m->g_lastts.as<int>(), st));
+    MB_TRY(decoder_prefill(m, rows, P, m->g_prefill_ids.as<long long>(), gp->position_rule, st));
+    MB_TRY(final_logits(m, rows, m->p_x.as<float>() + (size_t)(P - 1) * d, (long long)P * d, st, false));
+    MB_TRY(launch_beam_step(bp, B, st));
+
+    const int n_splits_self = self_splits(gp->max_length);
+    auto key = std::make_tuple(rows, (int)B, n_splits_self, K);
+    auto it = m->graphs.find(key);
+    if (it == m->graphs.end()) {
+        cudaGraph_t graph;
+        if (!m->cap_stream) MB_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
+        MB_CUDA_CHECK(cudaStreamSynchronize(st));
+        MB_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
+        const long long before = g_launch_count;
+        int s = token_step(m, rows, B, n_splits_self, m->cap_stream, m->use_pdl, nullptr, &bp);
+        cudaError_t e = cudaStreamEndCapture(m->cap_stream, &graph);
+        m->graph_nodes[key] = g_launch_count - before;
+        g_launch_count = before;
+        if (s) return s;
+        MB_CUDA_CHECK(e);
+        cudaGraphExec_t exec;
+        MB_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
+        cudaGraphDestroy(graph);
+        it = m->graphs.emplace(key, exec).first;
+    }
+    int remaining = gp->max_length - (P + 1);
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag, &m->g_state.as<GenState>()->all_finished, 4, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));
+    if (*m->h_flag) remaining = 0;
+    while (remaining > 0) {
+        const int burst = std::min(remaining, 16);
+        for (int i = 0; i < burst; ++i) MB_CUDA_CHECK(cudaGraphLaunch(it->second, st));
+        g_launch_count += (long long)burst * m->graph_nodes[key];
+        remaining -= burst;
+        MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag, &m->g_state.as<GenState>()->all_finished, 4, cudaMemcpyDeviceToHost, st));
+        MB_CUDA_CHECK(cudaStreamSynchronize(st));
+        if (*m->h_flag) break;
+    }
+    GenState fin{};
+    MB_CUDA_CHECK(cudaMemcpyAsync(&fin, m->g_state.p, sizeof(fin), cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));
+    // the finished store the last selection wrote (parity of the step count)
+    std::vector<long long> fids((size_t)BK * ids_ld);
+    std::vector<int> flen(BK);
+    std::vector<unsigned char> fflag(BK);
+    MB_CUDA_CHECK(cudaMemcpyAsync(fids.data(), m->b_finids[fin.step & 1].p, fids.size() * 8, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(finscore.data(), m->b_finscore.p, BK * 4, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(flen.data(), m->b_finlen.p, BK * 4, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(fflag.data(), m->b_finflag.p, BK, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));
+    // best hypothesis per item, padded to P + the longest generated length with the filler id
+    int gen_max = 0;
+    for (int b = 0; b < B; ++b) {
+        MB_REQUIRE(fflag[(size_t)b * K], "beam search ended without a finished hypothesis");
+        gen_max = std::max(gen_max, flen[(size_t)b * K]);
+    }
+    const int Lout = P + gen_max;
+    for (int b = 0; b < B; ++b) {
+        const long long* h = fids.data() + (size_t)b * K * ids_ld;
+        const int Lb = P + flen[(size_t)b * K];
+        for (int t = 0; t < Lout; ++t) out_ids[(size_t)b * Lout + t] = t < Lb ? h[t] : fill_id;
+        out_scores[b] = finscore[(size_t)b * K];
+    }
+    *out_len = Lout;
     return 0;
 }
 
@@ -1171,5 +1347,72 @@ extern "C" int mb200_model_logits_chain(mb200_model* m, const float* logits, int
     MB_CUDA_CHECK(cudaMemcpy2DAsync(chosen.data(), 8, m->g_ids.as<long long>() + L, (size_t)ids_ld * 8, 8, B, cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
     for (int b = 0; b < B; ++b) chosen_out[b] = chosen[b];
+    return 0;
+}
+
+// Parity hook for beam search (tests; not part of the reference-facing boundary): ONE selection step of the beam kernels on
+// caller-supplied logits, from an empty finished store.  logits DEVICE [rows, V] (rows = 2*B*K under CFG, negative-prompt rows first);
+// ids HOST [B*K, L] the running sequences; run_scores HOST [B*K]; `step` / `has_last_scores` as in mb200_model_logits_chain.
+// Outputs: logprobs_out DEVICE [B*K, V] = the processed log-probs (before the running score is added); HOST [B*K]: top_out = the first
+// K candidates of each item (flat index beam * V + token, in order), parent_out = the batch row each new running beam continues,
+// token_out / score_out = its token and running score, fin_score_out / fin_len_out / fin_flag_out = the finished store
+// (-1e9 / 0 / 0 where empty); fin_ids_out HOST [B*K, L + 1] its ids.
+extern "C" int mb200_model_beam_step(mb200_model* m, const float* logits, int32_t B, int32_t num_beams, int32_t use_cfg, const int64_t* ids,
+                                     int32_t L, int32_t prompt_len, const uint8_t* vflags, const mb200_generate_params* gp,
+                                     const float* run_scores, int32_t step, int32_t has_last_scores, float* logprobs_out, int32_t* top_out,
+                                     int32_t* parent_out, int64_t* token_out, float* score_out, float* fin_score_out, int32_t* fin_len_out,
+                                     uint8_t* fin_flag_out, int64_t* fin_ids_out, void* stream) {
+    MB_REQUIRE(m && m->finalized && logits && ids && vflags && gp && run_scores && logprobs_out && top_out && parent_out && token_out &&
+               score_out && fin_score_out && fin_len_out && fin_flag_out && fin_ids_out, "null argument");
+    const auto& c = m->cfg;
+    const int K = num_beams, BK = B * K, rows = use_cfg ? 2 * BK : BK, V = c.vocab_size_out, ids_ld = c.tgt_seq_len;
+    MB_REQUIRE(K >= 2 && K <= 4, "num_beams must be in [2, 4]");
+    MB_REQUIRE(B >= 1 && rows <= m->max_rows && prompt_len >= 1 && L >= prompt_len && L < ids_ld && L < gp->max_length, "bad batch / length");
+    MB_REQUIRE(beam_select_smem_bytes(K, V, ids_ld) <= 220 * 1024, "beam candidates do not fit shared memory");
+    cudaStream_t st = (cudaStream_t)stream;
+    MB_TRY(ensure_beam_buffers(m));
+    std::vector<long long> idsrow((size_t)BK * ids_ld, (long long)gp->pad_token_id);
+    for (int j = 0; j < BK; ++j)
+        for (int t = 0; t < L; ++t) idsrow[(size_t)j * ids_ld + t] = ids[(size_t)j * L + t];
+    GenState gs{};
+    gs.cur_len = L; gs.prompt_len = prompt_len; gs.max_length = gp->max_length; gs.min_new_tokens = gp->min_new_tokens;
+    gs.step = step; gs.has_last_scores = has_last_scores;
+    const SampleConfig sc = make_sample_config(gp, BK, use_cfg != 0, V, ids_ld);
+    std::vector<int> zeros(rows, 0);
+    std::vector<float> empty(BK, -1.0e9f);
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_ids.p, idsrow.data(), idsrow.size() * 8, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_vflags.p, vflags, c.vocab_size_in, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_state.p, &gs, sizeof(gs), cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_cfg.p, &sc, sizeof(sc), cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_leftpad.p, zeros.data(), rows * 4, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->b_kvsrc.p, 0, (size_t)rows * ids_ld * sizeof(int), st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->b_runscore.p, run_scores, BK * 4, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->b_finscore.p, empty.data(), BK * 4, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->b_finlen.p, 0, BK * sizeof(int), st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->b_finflag.p, 0, BK, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->b_unsat.p, 1, B, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->d_logits.p, logits, (size_t)rows * V * 4, cudaMemcpyDeviceToDevice, st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));
+    MB_TRY(launch_prompt_scan(m->g_ids.as<long long>(), ids_ld, BK, L, m->g_vflags.as<unsigned char>(), sc.ts_start, sc.ts_end,
+                              m->g_lastts.as<int>(), st));
+    BeamParams bp = beam_params(m, rows, K);
+    bp.dbg_logprobs = logprobs_out;
+    MB_TRY(m->b_dbg.ensure((size_t)2 * m->max_rows * sizeof(int)));
+    bp.dbg_top = m->b_dbg.as<int>(); bp.dbg_parent = m->b_dbg.as<int>() + m->max_rows;
+    MB_TRY(launch_beam_step(bp, B, st));
+    std::vector<int> dbg((size_t)2 * m->max_rows);
+    std::vector<long long> tok((size_t)BK * ids_ld), fids((size_t)BK * ids_ld);
+    MB_CUDA_CHECK(cudaMemcpyAsync(dbg.data(), m->b_dbg.p, dbg.size() * 4, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(tok.data(), m->g_ids.p, tok.size() * 8, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(fids.data(), m->b_finids[1 - (step & 1)].p, fids.size() * 8, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(score_out, m->b_runscore.p, BK * 4, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(fin_score_out, m->b_finscore.p, BK * 4, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(fin_len_out, m->b_finlen.p, BK * 4, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(fin_flag_out, m->b_finflag.p, BK, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int j = 0; j < BK; ++j) {
+        top_out[j] = dbg[j]; parent_out[j] = dbg[m->max_rows + j]; token_out[j] = tok[(size_t)j * ids_ld + L];
+        for (int t = 0; t <= L; ++t) fin_ids_out[(size_t)j * (L + 1) + t] = fids[(size_t)j * ids_ld + t];
+    }
     return 0;
 }

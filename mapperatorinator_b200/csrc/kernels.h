@@ -212,6 +212,7 @@ struct DecAttnParams {
     int rows, H, n_splits, chunk;
     float* out; long long out_ld;                   // merged heads [rows, H*64], written by the LAST split of each (row, head) to arrive
     int* ticket;                                    // [rows, H] arrival counters, zero on entry, reset by the last arriver
+    const int* kv_src; long long kv_src_ld;         // beam search: [rows, kv_src_ld] cache row holding key position t of row r (null = row r)
 };
 int launch_decode_attention(const DecAttnParams& p, cudaStream_t stream, bool pdl);
 
@@ -238,6 +239,25 @@ struct SampleParams {
     unsigned long long* trace;                      // tools/mega3_trace.py: clock64 stamps inside the selection phase (null in production)
 };
 int launch_sample(const SampleParams& p, int B, cudaStream_t stream, bool pdl);
+
+// ---- beam.cu: beam search (num_beams K <= 4) after the decoder's final logits ---------------------------------------------
+struct BeamParams {
+    SampleParams sample;                            // chain state with logits = logprobs, cfg->B = B*K beam rows, ids [B*K, ids_ld]
+    const float* logits; long long logits_ld;       // decoder logits [rows (2*B*K under CFG), V]
+    float* logprobs;                                // [rows, V] log_softmax of every decoder row
+    float* cand;                                    // [B*K, V] processed log-probs + running beam score
+    float* run_score;                               // [B*K] running beam scores
+    int* kv_src; long long kv_src_ld;               // [rows, kv_src_ld] self-attention source-row table
+    long long* fin_ids[2];                          // finished hypotheses [B*K, ids_ld], double-buffered by step parity
+    float* fin_score; int* fin_len; unsigned char* fin_flag;   // [B*K]: score, generated tokens, real hypothesis
+    unsigned char* unsat;                           // [B] early-stop heuristic not yet satisfied
+    int K, V, ids_ld;
+    float* dbg_logprobs;                            // parity hook, null in production: [B*K, V] processed log-probs
+    int* dbg_parent;                                // parity hook, null in production: [B*K] parent row of each new beam
+    int* dbg_top;                                   // parity hook, null in production: [B*K] first K candidates per item (flat index)
+};
+size_t beam_select_smem_bytes(int K, int V, int ids_ld);
+int launch_beam_step(const BeamParams& bp, int B, cudaStream_t stream);
 
 // ---- decode_mega.cu: the persistent token-loop megakernel ----------------------------------------------------------------
 constexpr int MEGA_WBUF_FLOATS = 19968;       // 78 KB per buffer, two buffers per CTA (one arena: see wslice in decode_mega.cu)

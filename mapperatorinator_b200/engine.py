@@ -156,10 +156,11 @@ class ModelEngine:
                  negative_mask: Optional[torch.Tensor] = None, position_rule: str = "arange") -> torch.Tensor:
         """The token loop of `server.model_generate` for rows whose encoder states already sit in `slots`.
         Returns a CPU LongTensor (B, L) = prompt + generated, like the reference."""
+        if int(generate_kwargs.get("num_beams", 1) or 1) != 1:
+            return self.generate_beams(slots, prompt, prompt_mask, layout, generate_kwargs, negative_prompt, negative_mask,
+                                       position_rule)[0]
         p, eos_ids, gk = self._generate_params(layout, generate_kwargs, position_rule)
         B, P = prompt.shape
-        if int(gk.get("num_beams", 1) or 1) != 1:
-            raise NotImplementedError("beam search is outside the hot path (SURVEY §8: greedy / sampling only)")
         use_cfg = negative_prompt is not None and p.cfg_scale > 1.0
 
         ids = np.ascontiguousarray(prompt.detach().cpu().numpy().astype(np.int64))
@@ -186,6 +187,53 @@ class ModelEngine:
         L = out_len.value
         return torch.from_numpy(out.reshape(-1)[: B * L].reshape(B, L).copy())
 
+    def generate_beams(self, slots: Sequence[int], prompt: torch.Tensor, prompt_mask: Optional[torch.Tensor], layout: TokenLayout,
+                       generate_kwargs: dict, negative_prompt: Optional[torch.Tensor] = None,
+                       negative_mask: Optional[torch.Tensor] = None, position_rule: str = "arange"):
+        """`generate` with HF beam search (`num_beams` = K in [2, 4], do_sample False, default length_penalty / early_stopping).
+        Returns (ids CPU LongTensor (B, L): the best finished hypothesis of each item, padded with `pad_token_id` or, when that
+        is 0, the first EOS id, like the reference; scores CPU FloatTensor (B,): HF's `sequences_scores`)."""
+        gk = dict(generate_kwargs)
+        K = int(gk.get("num_beams", 1) or 1)
+        if not 2 <= K <= 4:
+            raise ValueError(f"num_beams={K}: beam search takes 2..4 beams (the candidates of one item live in one CTA's shared memory)")
+        if gk.get("do_sample", False):
+            raise ValueError("do_sample with num_beams > 1 (beam sampling) is not supported")
+        if int(gk.get("num_return_sequences", 1) or 1) != 1:
+            raise ValueError("num_return_sequences != 1 is not supported")
+        if gk.get("length_penalty") not in (None, 1.0) or gk.get("early_stopping") not in (None, False):
+            raise ValueError("beam search supports only the default length_penalty (1.0) and early_stopping (False)")
+        p, eos_ids, gk = self._generate_params(layout, gk, position_rule)
+        B, P = prompt.shape
+        use_cfg = negative_prompt is not None and p.cfg_scale > 1.0
+        rows = B * K * (2 if use_cfg else 1)
+        if rows > self.max_batch:
+            raise ValueError(f"beam search needs batch * num_beams{' * 2 (classifier-free guidance)' if use_cfg else ''} = {rows} "
+                             f"decoder rows; this engine was built with max_batch={self.max_batch}")
+        ids = np.ascontiguousarray(prompt.detach().cpu().numpy().astype(np.int64))
+        msk = None if prompt_mask is None else np.ascontiguousarray(prompt_mask.detach().cpu().numpy().astype(np.uint8))
+        neg = nmsk = None
+        if use_cfg:
+            neg_full = ids.copy()
+            npn = negative_prompt.detach().cpu().numpy().astype(np.int64)
+            neg_full[:, :npn.shape[1]] = npn
+            neg = np.ascontiguousarray(neg_full)
+            nmsk = np.ascontiguousarray(msk.copy() if msk is not None else np.ones_like(ids, dtype=np.uint8))
+        vflags = build_vflags(layout, eos_ids)
+        slots_a = np.ascontiguousarray(np.asarray(list(slots), dtype=np.int32))
+        assert slots_a.shape[0] == B
+        fill = p.pad_token_id if p.pad_token_id else eos_ids[0]          # HF: `pad_token_id or eos_token_id[0]`
+        out = np.zeros((B, p.max_length), dtype=np.int64)
+        scores = np.zeros(B, dtype=np.float32)
+        out_len = C.c_int32(0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.mb200_model_generate_beams(
+                self.handle, slots_a.ctypes.data, B, ids.ctypes.data, None if msk is None else msk.ctypes.data, P,
+                None if neg is None else neg.ctypes.data, None if nmsk is None else nmsk.ctypes.data, vflags.ctypes.data,
+                C.byref(p), K, int(fill), out.ctypes.data, C.byref(out_len), scores.ctypes.data, _stream()))
+        L = out_len.value
+        return torch.from_numpy(out.reshape(-1)[: B * L].reshape(B, L).copy()), torch.from_numpy(scores)
+
     def logits_chain(self, logits: torch.Tensor, ids: torch.Tensor, prompt_len: int, layout: TokenLayout, generate_kwargs: dict,
                      step: int = 0, has_last_scores: bool = False, use_cfg: bool = False):
         """Parity hook: one selection step of the fused logits-processor chain on given logits (rows, V) CUDA f32 and ids (B, L).
@@ -202,6 +250,33 @@ class ModelEngine:
                                                          vflags.ctypes.data, C.byref(p), int(step), int(has_last_scores), scores.data_ptr(),
                                                          chosen.ctypes.data, _stream()))
         return scores, torch.from_numpy(chosen)
+
+    def beam_step(self, logits: torch.Tensor, ids: torch.Tensor, run_scores: torch.Tensor, num_beams: int, prompt_len: int,
+                  layout: TokenLayout, generate_kwargs: dict, step: int = 0, has_last_scores: bool = False, use_cfg: bool = False) -> dict:
+        """Parity hook: one beam-search selection step on given logits (rows, V) CUDA f32, running sequences ids (B*K, L) and running
+        scores (B*K,), from an empty finished store.  Returns a dict of CPU tensors: logprobs (B*K, V) processed log-probs, top (B*K)
+        the first K candidates per item as flat indices beam * V + token, parent / token / score (B*K) the new running beams
+        (parent = batch row), fin_score / fin_len / fin_flag (B*K) and fin_ids (B*K, L + 1) the finished store."""
+        p, eos_ids, gk = self._generate_params(layout, generate_kwargs)
+        BK, L = ids.shape
+        B = BK // num_beams
+        a = np.ascontiguousarray(ids.detach().cpu().numpy().astype(np.int64))
+        rs = np.ascontiguousarray(run_scores.detach().cpu().numpy().astype(np.float32))
+        vflags = build_vflags(layout, eos_ids)
+        logits = logits.contiguous().float()
+        lp = torch.empty(BK, self.cfg.vocab_size_out, device=logits.device, dtype=torch.float32)
+        out = dict(top=np.zeros(BK, np.int32), parent=np.zeros(BK, np.int32), token=np.zeros(BK, np.int64), score=np.zeros(BK, np.float32),
+                   fin_score=np.zeros(BK, np.float32), fin_len=np.zeros(BK, np.int32), fin_flag=np.zeros(BK, np.uint8),
+                   fin_ids=np.zeros((BK, L + 1), np.int64))
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.mb200_model_beam_step(
+                self.handle, logits.data_ptr(), B, int(num_beams), int(use_cfg), a.ctypes.data, L, int(prompt_len), vflags.ctypes.data,
+                C.byref(p), rs.ctypes.data, int(step), int(has_last_scores), lp.data_ptr(), out["top"].ctypes.data,
+                out["parent"].ctypes.data, out["token"].ctypes.data, out["score"].ctypes.data, out["fin_score"].ctypes.data,
+                out["fin_len"].ctypes.data, out["fin_flag"].ctypes.data, out["fin_ids"].ctypes.data, _stream()))
+        res = {k: torch.from_numpy(v) for k, v in out.items()}
+        res["logprobs"] = lp.cpu()
+        return res
 
     def forward_logits(self, slots: Sequence[int], ids: torch.Tensor, mask: Optional[torch.Tensor],
                        position_rule: str = "arange") -> torch.Tensor:
