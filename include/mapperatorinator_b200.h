@@ -120,6 +120,25 @@ int mb200_model_generate_beams(mb200_model* m, const int32_t* slots, int32_t bat
                                const mb200_generate_params* params, int32_t num_beams, int64_t fill_id, int64_t* out_ids,
                                int32_t* out_len, float* out_scores, void* cuda_stream);
 
+/* Ragged batched generate: n_req independent requests in ONE token loop.  Request r has its own prompt (no padding), its own
+ * generate params (max_length, min_new_tokens, EOS set and look-back range, temperatures, time-shift bias, sampling settings and
+ * seed, cfg_scale) and its own encoder slot; row r of the result is bit-identical in its ids to mb200_model_generate called with
+ * batch 1 for that request alone (positions 0..P_r-1 then P_r.., conditional temperature decided on the row itself, the sampling
+ * counter of batch row 0, stop on its own EOS set or max_length).  All arrays are HOST memory.
+ *   slots[n_req]                  encoder-state slot of each request
+ *   prompt / prompt_off           int64 prompt ids of all requests back to back; request r owns [prompt_off[r], prompt_off[r+1])
+ *   neg_prompt                    NULL, or the negative-prompt rows at the same offsets (the request's prompt with its leading tokens
+ *                                 replaced, as for mb200_model_generate).  Either every request has cfg_scale > 1 and a negative row
+ *                                 or none has: a mixed call is rejected.
+ *   vflags[n_req, vocab_size_in]  per-request token flags (only the EOS bits differ between requests)
+ *   params[n_req]                 per-request parameters; position_rule is not used (there is no padding)
+ *   out_ids[n_req, out_ld]        int64, prompt + generated of each request; out_len[n_req] = its length
+ * Rejected before anything is launched: more decoder rows than max_batch (n_req, doubled under CFG), prompt_len >= max_length,
+ * max_length > tgt_seq_len or out_ld, mixed CFG.  Beam search stays on mb200_model_generate_beams. */
+int mb200_model_generate_ragged(mb200_model* m, int32_t n_req, const int32_t* slots, const int64_t* prompt, const int32_t* prompt_off,
+                                const int64_t* neg_prompt, const uint8_t* vflags, const mb200_generate_params* params,
+                                int64_t* out_ids, int32_t out_ld, int32_t* out_len, void* cuda_stream);
+
 /* Mapperatorinator.forward teacher-forced logits (server.model_forward, server.py:159-181), no CFG mixing.
  * ids: HOST int64 [batch, len]; mask HOST uint8; logits_out: DEVICE f32 [batch, len, vocab_size_out]. */
 int mb200_model_forward_logits(mb200_model* m, const int32_t* slots, int32_t batch, const int64_t* ids, const uint8_t* mask,

@@ -19,18 +19,18 @@ namespace {
 
 constexpr int GEMV_THREADS = 128, GEMV_WARPS = GEMV_THREADS / 32;
 
-template <int NB>
+template <int NB, bool RAGGED = false>
 __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(GemvParams p) {
     extern __shared__ __align__(16) float xs[];   // [NB][K] activations, then 32 floats of LayerNorm reduction scratch
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     pdl_launch_dependents();
     pdl_wait();
-    const int cur_pos = p.st ? p.st->cur_len - 1 : 0;
+    const int cur_pos = (p.st && !RAGGED) ? p.st->cur_len - 1 : 0;
     for (int b0 = 0; b0 < p.B; b0 += NB) {
         gemv_stage_x<NB, GEMV_THREADS>(p, b0, xs, xs + NB * p.K, tid);
         __syncthreads();
         for (int n = blockIdx.x * GEMV_WARPS + warp; n < p.N; n += gridDim.x * GEMV_WARPS)
-            gemv_row<NB, true>(p, n, p.W + (long long)n * p.ldw, xs, b0, lane, cur_pos);
+            gemv_row<NB, true, RAGGED>(p, n, p.W + (long long)n * p.ldw, xs, b0, lane, cur_pos);
         __syncthreads();
     }
 }
@@ -65,12 +65,40 @@ __global__ void __launch_bounds__(256) decode_attention_warp_kernel(DecAttnParam
     decode_attention_warp_body(p, s, h, r, p.row_slot ? p.row_slot[r] : r, L, P, sc[warp], lane);
 }
 
+// Ragged self attention: the unit (split s, head h, row r) of the grid runs with the geometry of row r's OWN call — key count
+// cur_len_r, the split plan of max_length_r — so its partials and their merge order are that call's, bit for bit.  Splits of the grid
+// beyond the row's plan do not exist for it (no partial, no ticket); an empty split inside the plan contributes nothing, as always.
+// One instantiation with room for 128 keys: rows with the single 128-key split and rows with 64-key splits share a launch, and the
+// per-row geometry does not fit the 80 registers that give the uniform 64-key kernel its extra resident CTAs anyway.
+__global__ void __launch_bounds__(128, 4) decode_attention_ragged_kernel(DecAttnParams p) {
+    constexpr int KMAX = 128;
+    __shared__ float sc[128];
+    __shared__ float red[4][64];
+    __shared__ float stat[2];
+    pdl_launch_dependents();
+    pdl_wait();
+    const int s = blockIdx.x, h = blockIdx.y, r = blockIdx.z;
+    const RowState* rs = ragged_rows(p.st) + r % p.st->n_req;
+    const int L = rs->cur_len;
+    const int S = self_splits(rs->max_length);
+    if (s >= S) return;                                // uniform across the CTA
+    // partials stay at (row, head) stride p.n_splits while the body indexes them with the row's own split count
+    const long long shift = ((long long)r * p.H + h) * (p.n_splits - S);
+    p.part_o += shift * 64; p.part_ml += shift * 2;
+    p.n_splits = S;
+    p.chunk = S == 1 ? 128 : 64;
+    AttnRegs<4, KMAX> regs;
+    decode_attention_load<4, KMAX, false>(p, s, h, r, r, L, 0, threadIdx.x, regs);
+    decode_attention_body<4, KMAX, false>(p, s, h, r, r, L, 0, sc, red, stat, threadIdx.x, regs);
+}
+
+template <bool RAGGED>
 __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleParams p) {
     __shared__ SampleSmem sm;
     pdl_launch_dependents();
     pdl_wait();
     if (p.st->all_finished) return;   // replays past the end of a call are no-ops (uniform across the grid)
-    sample_body<SAMPLE_THREADS>(p, blockIdx.x, sm);
+    sample_body<SAMPLE_THREADS, RAGGED>(p, blockIdx.x, sm);
 }
 
 __global__ void prompt_scan_kernel(const long long* ids, long long ids_ld, int P, const unsigned char* vflags, int ts_start, int ts_end,
@@ -81,6 +109,21 @@ __global__ void prompt_scan_kernel(const long long* ids, long long ids_ld, int P
     for (int t = 0; t < P; ++t) {
         long long tok = ids[(long long)b * ids_ld + t];
         if (vflags[tok] & VF_SOS) lt = -1;
+        else if (tok >= ts_start && tok < ts_end) lt = (int)(tok - ts_start);
+    }
+    last_ts[b] = lt;
+}
+
+__global__ void prompt_scan_ragged_kernel(const long long* ids, long long ids_ld, const GenState* st, const unsigned char* vflags, long long vflags_ld,
+                                          int ts_start, int ts_end, int* last_ts) {
+    const int b = blockIdx.x;
+    if (threadIdx.x != 0) return;
+    const int P = ragged_rows(st)[b].prompt_len;
+    const unsigned char* vf = vflags + b * vflags_ld;
+    int lt = -1;
+    for (int t = 0; t < P; ++t) {
+        long long tok = ids[(long long)b * ids_ld + t];
+        if (vf[tok] & VF_SOS) lt = -1;
         else if (tok >= ts_start && tok < ts_end) lt = (int)(tok - ts_start);
     }
     last_ts[b] = lt;
@@ -123,7 +166,7 @@ int launch_with_attrs(Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_
 
 }  // namespace
 
-int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl) {
+int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged) {
     MB_REQUIRE(p.K % 4 == 0 && p.ldw % 4 == 0, "GEMV K / ldw must be multiples of 4");
     MB_REQUIRE(p.xmode != X_LAYERNORM || p.K <= 1024, "fused LayerNorm prologue supports K <= 1024");
     if (p.B <= 0 || p.N <= 0) return 0;
@@ -136,10 +179,23 @@ int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl) {
         MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         configured = true;
     }
     MB_REQUIRE(smem <= 200 * 1024, "GEMV activation tile does not fit shared memory");
     g_prof_class = 0;
+    if (ragged) {
+        MB_REQUIRE(p.st, "ragged GEMV needs the ragged state");
+        switch (nb) {
+            case 1: return launch_with_attrs(gemv_kernel<1, true>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
+            case 2: return launch_with_attrs(gemv_kernel<2, true>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
+            case 4: return launch_with_attrs(gemv_kernel<4, true>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
+            default: return launch_with_attrs(gemv_kernel<8, true>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
+        }
+    }
     switch (nb) {
         case 1: return launch_with_attrs(gemv_kernel<1>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
         case 2: return launch_with_attrs(gemv_kernel<2>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
@@ -170,14 +226,30 @@ int launch_decode_attention(const DecAttnParams& p, cudaStream_t stream, bool pd
     return launch_with_attrs(decode_attention_kernel<128>, dim3(p.n_splits, p.H, p.rows), dim3(128), 0, stream, pdl, p);
 }
 
-int launch_sample(const SampleParams& p, int B, cudaStream_t stream, bool pdl) {
+int launch_decode_attention_ragged(const DecAttnParams& p, cudaStream_t stream, bool pdl) {
+    MB_REQUIRE(p.st && p.out && p.ticket && !p.kv_src && p.fixed_len == 0, "ragged decode attention is the self attention of a ragged state");
+    if (p.rows <= 0) return 0;
+    g_prof_class = 1;
+    return launch_with_attrs(decode_attention_ragged_kernel, dim3(p.n_splits, p.H, p.rows), dim3(128), 0, stream, pdl, p);
+}
+
+int launch_sample(const SampleParams& p, int B, cudaStream_t stream, bool pdl, bool ragged) {
     g_prof_class = 2;
-    return launch_with_attrs(sample_kernel, dim3(B), dim3(SAMPLE_THREADS), 0, stream, pdl, p);
+    if (ragged) return launch_with_attrs(sample_kernel<true>, dim3(B), dim3(SAMPLE_THREADS), 0, stream, pdl, p);
+    return launch_with_attrs(sample_kernel<false>, dim3(B), dim3(SAMPLE_THREADS), 0, stream, pdl, p);
 }
 
 int launch_prompt_scan(const long long* ids, long long ids_ld, int B, int P, const unsigned char* vflags, int ts_start, int ts_end,
                        int* last_ts, cudaStream_t stream) {
     prompt_scan_kernel<<<B, 32, 0, stream>>>(ids, ids_ld, P, vflags, ts_start, ts_end, last_ts);
+    MB_LAUNCH_CHECK();
+    ++g_launch_count;
+    return 0;
+}
+
+int launch_prompt_scan_ragged(const long long* ids, long long ids_ld, int B, const GenState* st, const unsigned char* vflags, long long vflags_ld,
+                              int ts_start, int ts_end, int* last_ts, cudaStream_t stream) {
+    prompt_scan_ragged_kernel<<<B, 32, 0, stream>>>(ids, ids_ld, st, vflags, vflags_ld, ts_start, ts_end, last_ts);
     MB_LAUNCH_CHECK();
     ++g_launch_count;
     return 0;

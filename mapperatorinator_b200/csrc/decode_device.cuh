@@ -219,7 +219,9 @@ __device__ __forceinline__ float gemv_dot(int K, const float* wrow_f, const floa
     return mine;
 }
 
-template <int NB, bool W_GLOBAL>
+// RAGGED (p.st heads a ragged state, `cur_pos` unused): a segment with pos_stride writes row b at the row's own cache position, and
+// leaves the cache of a finished row alone.
+template <int NB, bool W_GLOBAL, bool RAGGED = false>
 __device__ __forceinline__ void gemv_row(const GemvParams& p, int n, const float* wrow_f, const float* xs, int b0, int lane, int cur_pos,
                                          bool have_operands = false, float bias_v = 0.f, float r_v = 0.f, unsigned long long* dbg = nullptr) {
     if (!have_operands) gemv_row_operands<NB>(p, n, b0, lane, bias_v, r_v);
@@ -228,6 +230,12 @@ __device__ __forceinline__ void gemv_row(const GemvParams& p, int n, const float
     const int bl = min(b0 + (lane < NB ? lane : 0), p.B - 1);
     const int si = (int)(p.nseg > 1 && n >= p.seg[1].n_begin) + (int)(p.nseg > 2 && n >= p.seg[2].n_begin);
     const GemvSeg& sg = p.seg[si];
+    bool live = true;
+    if (RAGGED) {
+        const RowState* rs = ragged_rows(p.st) + bl % ld_state(&p.st->n_req);
+        cur_pos = ld_state(&rs->cur_len) - 1;
+        live = sg.pos_stride == 0 || ld_state(&rs->finished) == 0;
+    }
     float* const outp = sg.out + ((long long)bl * sg.out_bs + (long long)cur_pos * sg.pos_stride + (n - sg.n_begin));
     const int act = sg.act;
     const float alpha = sg.alpha;
@@ -238,7 +246,7 @@ __device__ __forceinline__ void gemv_row(const GemvParams& p, int n, const float
         if (has_bias) v += bias_v;
         v = apply_act(v, act) * alpha;
         if (has_res) v += r_v;
-        *outp = v;
+        if (!RAGGED || live) *outp = v;
     }
 }
 
@@ -877,16 +885,26 @@ static __device__ __forceinline__ int sample_greedy_regs(const SampleParams& p, 
     return bi == 0x7fffffff ? 0 : bi;
 }
 
+// vocabulary flags of batch row b: the call's one table, or the row's own in a ragged call (re-derived at every use: a pointer kept
+// live across the chain costs the uniform instantiations a register)
+template <bool RAGGED>
+static __device__ __forceinline__ const unsigned char* row_vflags(const SampleParams& p, const SampleConfig& c, int b) {
+    if (RAGGED) return p.vflags + (long long)b * c.vflags_ld;
+    return p.vflags;
+}
+
 // The logits-processor chain of one batch row b (steps 0-5: min_new_tokens EOS mask, CFG, MonotonicTimeShift, TimeshiftBias,
 // temperature decided on row 0, LookbackBias) from p.logits into sm.s.  Shared by the token selection below (on logits) and by the
 // beam-search scores phase (beam.cu, on log-probs).
-template <int NT>
+// RAGGED (mb200_model_generate_ragged): row b is its own batch-1 call — its own SampleConfig and vocabulary-flag row, and the
+// conditional temperature decided on ITS last tokens (in a batch-1 call, "row 0" is the row itself).
+template <int NT, bool RAGGED = false>
 static __device__ __forceinline__ void logits_chain(const SampleParams& p, int b, SampleSmem& sm, int L, int st_step, int st_has_last,
                                                     bool suppress_eos) {
     float* s = sm.s;
     float* scratch = sm.scratch;
     const int tid = threadIdx.x;
-    const SampleConfig& c = *p.cfg;
+    const SampleConfig& c = p.cfg[RAGGED ? b : 0];
     const int V = c.V, B = c.B;
     long long* ids_row = p.ids + (long long)b * c.ids_ld;
     // (0)+(1): min_new_tokens EOS suppression, then classifier-free guidance on raw logits
@@ -895,7 +913,7 @@ static __device__ __forceinline__ void logits_chain(const SampleParams& p, int b
     } else {
     _Pragma("unroll 1") for (int v = tid; v < V; v += NT) {
         float x;
-        const bool eos = (p.vflags[v] & VF_EOS) != 0;
+        const bool eos = (row_vflags<RAGGED>(p, c, b)[v] & VF_EOS) != 0;
         if (c.use_cfg) {
             float cond = __ldcg(p.logits + (long long)b * p.logits_ld + v);          // first half = "conditional" in HF's processor
             float unc = __ldcg(p.logits + (long long)(B + b) * p.logits_ld + v);
@@ -914,8 +932,8 @@ static __device__ __forceinline__ void logits_chain(const SampleParams& p, int b
         for (int i = 0; i < c.n_cond; ++i) {
             const int off = c.cond_offset[i];
             if (L >= off) {
-                long long t0 = __ldcg(p.ids + (L - off));   // row 0
-                if (t0 >= 0 && (p.vflags[t0] & c.cond_flag[i])) { temp = c.cond_temp[i]; break; }
+                long long t0 = __ldcg((RAGGED ? ids_row : p.ids) + (L - off));   // row 0 of the call
+                if (t0 >= 0 && (row_vflags<RAGGED>(p, c, b)[t0] & c.cond_flag[i])) { temp = c.cond_temp[i]; break; }
             }
         }
     }
@@ -940,7 +958,7 @@ static __device__ __forceinline__ void logits_chain(const SampleParams& p, int b
             const float* ls_prev = p.last_scores + ((long long)((st_step + 1) & 1) * B + b) * V;
             _Pragma("unroll 1") for (int v = tid; v < V; v += NT) ls_cur[v] = s[v];
             const long long last_tok = L > 0 ? __ldcg(ids_row + (L - 1)) : -1;
-            const bool timed = last_tok >= 0 && (p.vflags[last_tok] & VF_TIMED);
+            const bool timed = last_tok >= 0 && (row_vflags<RAGGED>(p, c, b)[last_tok] & VF_TIMED);
             if (st_has_last && timed) {
                 float m_last = -INFINITY, m_cur = -INFINITY;
                 _Pragma("unroll 1") for (int v = tid; v < V; v += NT) { m_last = fmaxf(m_last, __ldcg(ls_prev + v)); m_cur = fmaxf(m_cur, s[v]); }
@@ -951,7 +969,7 @@ static __device__ __forceinline__ void logits_chain(const SampleParams& p, int b
                     float pl = expf(__ldcg(ls_prev + v) - m_last);
                     float pc = expf(s[v] - m_cur);
                     z_last += pl; z_cur += pc;
-                    if (p.vflags[v] & VF_LB_EOS) e_last += pl;
+                    if (row_vflags<RAGGED>(p, c, b)[v] & VF_LB_EOS) e_last += pl;
                     if (!(v >= c.lookback_start && v < c.lookback_end)) o_cur += pc;
                 }
                 z_last = block_reduce<NT>(z_last, false, scratch);
@@ -981,28 +999,36 @@ static __device__ __forceinline__ void logits_chain(const SampleParams& p, int b
 // so this is about code size and register pressure of the caller, not about the 32 KB L1.5 instruction cache.)
 // Returns after the "last CTA" bookkeeping; the caller decides how the grid synchronises afterwards.
 // NT = threads of the calling CTA (512 in the per-phase kernel and the barrier megakernel, 256 in the dataflow megakernel).
-template <int NT>
+// RAGGED: lengths, limits and the finished flag are row b's own (ragged_rows(st)[b]); the draw uses row index 0 in its counter, as the
+// row's batch-1 call would; a finished row is frozen (nothing appended, its last embedding re-issued so the residual stream stays put).
+template <int NT, bool RAGGED = false>
 static __device__ __noinline__ void sample_body(const SampleParams& p, int b, SampleSmem& sm) {
     float* s = sm.s;
     int* sidx = sm.sidx;
     float* scratch = sm.scratch;
     const int tid = threadIdx.x;
-    const SampleConfig& c = *p.cfg;
+    const SampleConfig& c = p.cfg[RAGGED ? b : 0];
     GenState* st = p.st;
+    RowState* rs = ragged_rows(st) + b;                    // RAGGED only
     const int V = c.V, B = c.B;
-    const int L = ld_state(&st->cur_len);
-    const int st_prompt_len = ld_state(&st->prompt_len), st_min_new = ld_state(&st->min_new_tokens);
-    const int st_step = ld_state(&st->step), st_has_last = ld_state(&st->has_last_scores), st_max_length = ld_state(&st->max_length);
+    const int L = ld_state(RAGGED ? &rs->cur_len : &st->cur_len);
+    const int st_prompt_len = ld_state(RAGGED ? &rs->prompt_len : &st->prompt_len);
+    const int st_min_new = ld_state(RAGGED ? &rs->min_new_tokens : &st->min_new_tokens);
+    const int st_step = ld_state(&st->step), st_has_last = ld_state(&st->has_last_scores);
+    const int st_max_length = ld_state(RAGGED ? &rs->max_length : &st->max_length);
     long long* ids_row = p.ids + (long long)b * c.ids_ld;
     const bool suppress_eos = st_min_new > 0 && (L - st_prompt_len) < st_min_new;
 
     if (p.trace && tid == 0) p.trace[6] = (unsigned long long)clock64();
     int chosen = 0;
-    const bool fast_greedy = p.ll_logits != nullptr && !c.do_sample && p.dbg_scores == nullptr && V <= VMAX;
-    if (fast_greedy) {
+    const bool frozen = RAGGED && ld_state(&rs->finished) != 0;      // uniform across the CTA
+    const bool fast_greedy = !RAGGED && p.ll_logits != nullptr && !c.do_sample && p.dbg_scores == nullptr && V <= VMAX;
+    if (frozen) {
+        chosen = (int)__ldcg(ids_row + (L - 1));
+    } else if (fast_greedy) {
         chosen = sample_greedy_regs<NT>(p, b, sm, L, st_step, st_has_last, suppress_eos);
     } else {
-    logits_chain<NT>(p, b, sm, L, st_step, st_has_last, suppress_eos);
+    logits_chain<NT, RAGGED>(p, b, sm, L, st_step, st_has_last, suppress_eos);
 
     // (6)-(7) selection
     if (!c.do_sample) {
@@ -1124,7 +1150,7 @@ static __device__ __noinline__ void sample_body(const SampleParams& p, int b, Sa
             if (tid * SEG + j == first_keep - 1) scratch[33] = base + loc[j];
         __syncthreads();
         const float below = scratch[33];
-        const unsigned long long r = splitmix64(c.seed ^ splitmix64(((unsigned long long)st_step << 20) ^ (unsigned long long)b));
+        const unsigned long long r = splitmix64(c.seed ^ splitmix64(((unsigned long long)st_step << 20) ^ (unsigned long long)(RAGGED ? 0 : b)));
         const float u = below + (float)((r >> 40) + 0.5) * (1.0f / 16777216.0f) * (z - below);
         float cnt = 0.f;
 #pragma unroll
@@ -1142,15 +1168,18 @@ static __device__ __noinline__ void sample_body(const SampleParams& p, int b, Sa
 
     if (p.trace && tid == 0) p.trace[3] = (unsigned long long)clock64();
     // (8) finished rows emit pad; append; EOS test; state updates; next-step embedding
-    const bool was_finished = p.finished[b] != 0;
+    const bool was_finished = RAGGED ? false : p.finished[b] != 0;
     const long long tok = was_finished ? (long long)c.pad_id : (long long)chosen;
     __syncthreads();
-    if (tid == 0) {
+    if (tid == 0 && !frozen) {
         ids_row[L] = tok;
-        bool fin = was_finished || ((p.vflags[tok] & VF_EOS) != 0) || (L + 1 >= st_max_length);
-        if (fin && !was_finished) { p.finished[b] = 1; atomicAdd(&st->n_finished, 1); }
+        bool fin = was_finished || ((row_vflags<RAGGED>(p, c, b)[tok] & VF_EOS) != 0) || (L + 1 >= st_max_length);
+        if (RAGGED) {
+            rs->cur_len = L + 1;
+            if (fin) { rs->finished = 1; atomicAdd(&st->n_finished, 1); }
+        } else if (fin && !was_finished) { p.finished[b] = 1; atomicAdd(&st->n_finished, 1); }
         // MonotonicTimeShift state (logit_processors.py:149-166): last time shift after the last SOS-type token
-        const unsigned char fl = p.vflags[tok];
+        const unsigned char fl = row_vflags<RAGGED>(p, c, b)[tok];
         if (fl & VF_SOS) p.last_ts[b] = -1;
         else if (tok >= c.ts_start && tok < c.ts_end) p.last_ts[b] = (int)(tok - c.ts_start);
     }
@@ -1158,8 +1187,8 @@ static __device__ __noinline__ void sample_body(const SampleParams& p, int b, Sa
     const int nrep = c.use_cfg ? 2 : 1;
     for (int rep = 0; rep < nrep; ++rep) {
         const int row = rep * B + b;
-        int pos = L;
-        if (c.pos_rule_cumsum && p.n_left_pad) pos = L - p.n_left_pad[row];
+        int pos = frozen ? L - 1 : L;
+        if (!RAGGED && c.pos_rule_cumsum && p.n_left_pad) pos = L - p.n_left_pad[row];
         const float4* te = reinterpret_cast<const float4*>(p.tok_emb + tok * p.d_model);
         const float4* pe = reinterpret_cast<const float4*>(p.pos_emb + (long long)pos * p.d_model);
         float4* xo = reinterpret_cast<float4*>(p.x_out + (long long)row * p.x_ld);
@@ -1183,13 +1212,13 @@ static __device__ __noinline__ void sample_body(const SampleParams& p, int b, Sa
         // synchronise on the tag, not on the fences); the plain state for the host / the per-phase kernels follows.
         if (B > 1) __threadfence();                    // this row's n_finished update before its ticket
         if (atomicAdd(&st->ticket, 1) == B - 1) {
-            const int fin_all = (ld_state(&st->n_finished) >= B || L + 1 >= st_max_length) ? 1 : 0;
+            const int fin_all = (ld_state(&st->n_finished) >= B || (!RAGGED && L + 1 >= st_max_length)) ? 1 : 0;
             if (p.ll_hdr) {        // token header of the dataflow megakernel: next cur_len, all-finished flag
                 ll_store(p.ll_hdr + 0, __int_as_float(L + 1), p.ll_out_tag);
                 ll_store(p.ll_hdr + 1, __int_as_float(fin_all), p.ll_out_tag);
             }
             st->ticket = 0;
-            st->cur_len = L + 1;
+            if (!RAGGED) st->cur_len = L + 1;
             st->step = st_step + 1;
             st->has_last_scores = 1;
             if (fin_all) st->all_finished = 1;

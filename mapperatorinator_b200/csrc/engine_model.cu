@@ -326,14 +326,15 @@ extern "C" int mb200_model_finalize(mb200_model* m) {
     m->max_rows = std::max(1, c.max_batch);
     MB_TRY(m->cross_kv.ensure((size_t)c.decoder_layers * m->cross_layer_stride() * sizeof(float)));
     MB_TRY(m->self_kv.ensure((size_t)c.decoder_layers * m->self_layer_stride() * sizeof(float)));
-    MB_TRY(m->g_state.ensure(sizeof(GenState)));
-    MB_TRY(m->g_cfg.ensure(sizeof(SampleConfig)));
-    MB_TRY(m->g_vflags.ensure(c.vocab_size_in));
+    // sized for a ragged call (GenState + one RowState / SampleConfig / flag row per request); a uniform call uses element 0
+    MB_TRY(m->g_state.ensure(sizeof(GenState) + (size_t)m->max_rows * sizeof(RowState)));
+    MB_TRY(m->g_cfg.ensure((size_t)m->max_rows * sizeof(SampleConfig)));
+    MB_TRY(m->g_vflags.ensure((size_t)m->max_rows * c.vocab_size_in));
     MB_TRY(m->g_ids.ensure((size_t)m->max_rows * c.tgt_seq_len * sizeof(long long)));
     MB_TRY(m->g_prefill_ids.ensure((size_t)m->max_rows * c.tgt_seq_len * sizeof(long long)));
     MB_TRY(m->g_keyvalid.ensure((size_t)m->max_rows * c.tgt_seq_len));
     MB_TRY(m->g_leftpad.ensure(m->max_rows * sizeof(int)));
-    MB_TRY(m->g_rowslot.ensure(m->max_rows * sizeof(int)));
+    MB_TRY(m->g_rowslot.ensure((size_t)3 * m->max_rows * sizeof(int)));   // [max_rows] decode rows, then one (slot, slot) pair per request for ragged prefills
     MB_TRY(m->g_finished.ensure(m->max_rows));
     MB_TRY(m->g_lastts.ensure(m->max_rows * sizeof(int)));
     MB_TRY(m->g_lastscores.ensure((size_t)2 * m->max_rows * c.vocab_size_out * sizeof(float)));
@@ -512,8 +513,10 @@ extern "C" int mb200_model_encode(mb200_model* m, const float* pcm, int32_t n_wi
 // decoder prefill (shared by generate and forward_logits)
 // =====================================================================================================================
 // ids_dev [rows, P] int64, keyvalid_dev [rows, P], row_slot dev; afterwards p_x holds the final hidden states [rows*P, d]
-// (pre final-LN) and the self cache holds positions [0, P).
-static int decoder_prefill(mb200_model* m, int rows, int P, const long long* ids_dev, int pos_rule, cudaStream_t st) {
+// (pre final-LN) and the self cache holds positions [0, P).  Row i of the prefill writes self-cache row cache_row0 + i * cache_row_step
+// and reads the encoder slot row_slot[i] (defaults: cache rows 0.., the call's slot table).
+static int decoder_prefill(mb200_model* m, int rows, int P, const long long* ids_dev, int pos_rule, cudaStream_t st, int cache_row0 = 0,
+                           int cache_row_step = 1, const int* row_slot = nullptr) {
     const auto& c = m->cfg;
     const int d = c.d_model, f = c.ffn_dim, H = c.heads, T = c.src_seq_len / 2;
     const size_t RP = (size_t)rows * P;
@@ -521,12 +524,12 @@ static int decoder_prefill(mb200_model* m, int rows, int P, const long long* ids
     MB_TRY(m->p_attn.ensure(RP * d * 4)); MB_TRY(m->p_ffn.ensure(RP * f * 4));
     float *x = m->p_x.as<float>(), *h = m->p_h.as<float>(), *q = m->p_q.as<float>(), *att = m->p_attn.as<float>(), *ffn = m->p_ffn.as<float>();
     const unsigned char* kv_valid = m->g_keyvalid.as<unsigned char>();
-    const int* row_slot = m->g_rowslot.as<int>();
+    if (!row_slot) row_slot = m->g_rowslot.as<int>();
     MB_TRY(launch_embed(ids_dev, P, rows, rows, P, m->g_leftpad.as<int>(), pos_rule, m->tok_emb, m->dec_pos, d, x, st));
-    const long long self_row = (long long)c.tgt_seq_len * 2 * d;
+    const long long self_row = (long long)c.tgt_seq_len * 2 * d * cache_row_step;
     for (int l = 0; l < c.decoder_layers; ++l) {
         const LayerW& w = m->dec[l];
-        float* skv = m->self_kv.as<float>() + (size_t)l * m->self_layer_stride();
+        float* skv = m->self_kv.as<float>() + (size_t)l * m->self_layer_stride() + (size_t)cache_row0 * c.tgt_seq_len * 2 * d;
         const float* ckv = m->cross_kv.as<float>() + (size_t)l * m->cross_layer_stride();
         MB_TRY(layernorm(x, h, w.ln1_w, w.ln1_b, (int)RP, d, 1e-5f, st));
         MB_TRY(launch_gemm(gemm_base(plain_map(h, d), w.wqkv, d, plain_map(q, d), w.bqkv, (int)RP, d, d), st, &m->gemm));
@@ -608,15 +611,13 @@ static SampleParams sample_params(mb200_model* m, int rows) {
     return s;
 }
 
-// split-KV layout of the self-attention cache: one 128-key split while the context fits, 64-key splits beyond
-static int self_splits(int max_length) { return max_length <= 128 ? 1 : (max_length + 63) / 64; }
-
 // Either launches the 98 micro-phases of one token on `st` (eager / graph capture), or — when `collect` is given — records
 // them as phase descriptors for the persistent megakernel.  One definition, so both paths run the same arithmetic.
+// ragged: the step of a ragged call (per-phase kernels only) — n_splits_self is then the largest self-attention plan of the call.
 static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaStream_t st, bool pdl,
-                      std::vector<MegaPhase>* collect = nullptr, const BeamParams* beam = nullptr) {
+                      std::vector<MegaPhase>* collect = nullptr, const BeamParams* beam = nullptr, bool ragged = false) {
     auto emit_gemv = [&](const GemvParams& g) -> int {
-        if (!collect) return launch_gemv(g, st, pdl);
+        if (!collect) return launch_gemv(g, st, pdl, ragged && g.nseg > 1);      // only the cache-writing GEMV reads the row's position
         MegaPhase ph{}; ph.kind = 0; ph.g = g; collect->push_back(ph);
         return 0;
     };
@@ -657,6 +658,10 @@ static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaSt
             a.chunk = n_splits_self == 1 ? 128 : chunk;      // contexts up to 128 tokens: one split per head, no merge step
             a.out = attn; a.out_ld = d; a.ticket = ticket;
             if (beam) { a.kv_src = beam->kv_src; a.kv_src_ld = beam->kv_src_ld; }
+            if (ragged) {
+                a.key_valid = nullptr;      // no pad keys in a ragged row
+                MB_TRY(launch_decode_attention_ragged(a, st, pdl));
+            } else
             MB_TRY(emit_attn(a));
         }
         {   // out_proj + residual (the heads were merged by the attention phase)
@@ -714,7 +719,7 @@ static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaSt
         return 0;
     }
     if (beam) return launch_beam_step(*beam, B, st);
-    MB_TRY(launch_sample(sample_params(m, rows), B, st, pdl));
+    MB_TRY(launch_sample(sample_params(m, rows), B, st, pdl, ragged));
     return 0;
 }
 
@@ -852,7 +857,7 @@ static SampleConfig make_sample_config(const mb200_generate_params* gp, int B, b
     for (int i = 0; i < 3; ++i) { sc.cond_temp[i] = gp->cond_temp[i]; sc.cond_offset[i] = gp->cond_offset[i]; sc.cond_flag[i] = gp->cond_flag[i]; }
     sc.lookback_on = gp->lookback_on; sc.lookback_start = gp->lookback_start; sc.lookback_end = gp->lookback_end;
     sc.do_sample = gp->do_sample; sc.top_k = gp->top_k; sc.top_p = gp->top_p; sc.top_p_cut = gp->top_p_cut; sc.seed = gp->seed; sc.pad_id = gp->pad_token_id;
-    sc.pos_rule_cumsum = gp->position_rule; sc.ids_ld = ids_ld;
+    sc.pos_rule_cumsum = gp->position_rule; sc.ids_ld = ids_ld; sc.vflags_ld = 0;
     return sc;
 }
 
@@ -1023,6 +1028,134 @@ extern "C" int mb200_model_generate(mb200_model* m, const int32_t* slots, int32_
     MB_CUDA_CHECK(cudaMemcpy2DAsync(out_ids, (size_t)L * 8, m->g_ids.p, (size_t)ids_ld * 8, (size_t)L * 8, B, cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
     *out_len = L;
+    return 0;
+}
+
+// =====================================================================================================================
+// Ragged batched generate: n_req INDEPENDENT requests in one token loop, each row bit-identical in its ids to its own batch-1
+// mb200_model_generate call.  Prefill runs per request with the shapes of that call (1 row, 2 under classifier-free guidance) straight
+// into the request's cache rows; the first selection and every later token step run all rows together through the ragged per-phase
+// kernels (own length, own split plan, own processor settings, own EOS set per row), one CUDA-graph replay per token.  The two
+// megakernels stay uniform (rows <= 2).  Every bound is checked here, before anything is launched.
+extern "C" int mb200_model_generate_ragged(mb200_model* m, int32_t n_req, const int32_t* slots, const int64_t* prompt, const int32_t* prompt_off,
+                                           const int64_t* neg_prompt, const uint8_t* vflags, const mb200_generate_params* params,
+                                           int64_t* out_ids, int32_t out_ld, int32_t* out_len, void* stream) {
+    MB_REQUIRE(m && m->finalized, "model not finalized");
+    MB_REQUIRE(slots && prompt && prompt_off && vflags && params && out_ids && out_len, "null argument");
+    const auto& c = m->cfg;
+    cudaStream_t st = (cudaStream_t)stream;
+    const bool use_cfg = neg_prompt != nullptr;
+    const int N = n_req, rows = use_cfg ? 2 * N : N, nr = use_cfg ? 2 : 1;
+    MB_REQUIRE(N >= 1 && rows <= m->max_rows, "requests exceed max_batch (rows double under classifier-free guidance)");
+    MB_REQUIRE(prompt_off[0] == 0, "prompt offsets start at 0");
+    const int d = c.d_model, V = c.vocab_size_out, ids_ld = c.tgt_seq_len, Vin = c.vocab_size_in;
+    int n_splits_grid = 1, remaining = 0, first_poll = c.tgt_seq_len;
+    for (int r = 0; r < N; ++r) {
+        const mb200_generate_params& gp = params[r];
+        const int P = prompt_off[r + 1] - prompt_off[r];
+        MB_REQUIRE(P >= 1 && P < gp.max_length && gp.max_length <= c.tgt_seq_len, "need 1 <= prompt_len < max_length <= tgt_seq_len for every request");
+        MB_REQUIRE(gp.max_length <= out_ld, "output rows are shorter than a request's max_length");
+        MB_REQUIRE(slots[r] >= 0 && slots[r] < c.max_windows, "encoder slot out of range");
+        MB_REQUIRE((gp.cfg_scale > 1.0f) == use_cfg, "classifier-free guidance on every request of a ragged call or on none");
+        for (int t = prompt_off[r]; t < prompt_off[r + 1]; ++t) {
+            MB_REQUIRE(prompt[t] >= 0 && prompt[t] < Vin, "prompt token id out of range");
+            MB_REQUIRE(!use_cfg || (neg_prompt[t] >= 0 && neg_prompt[t] < Vin), "negative prompt token id out of range");
+        }
+        n_splits_grid = std::max(n_splits_grid, self_splits(gp.max_length));
+        remaining = std::max(remaining, gp.max_length - (P + 1));
+        first_poll = std::min(first_poll, std::min(std::max(gp.min_new_tokens, 1), gp.max_length - P));      // no row can stop earlier
+    }
+
+    // ---- host-side staging of the call state: one prompt per cache row, no padding anywhere ----
+    const int total = prompt_off[N];
+    std::vector<long long> pre((size_t)nr * total), idsrow((size_t)N * ids_ld, 0);
+    std::vector<size_t> pre_off(N);
+    std::vector<int> rowslot((size_t)3 * m->max_rows, 0);
+    std::vector<unsigned char> state(sizeof(GenState) + (size_t)N * sizeof(RowState), 0);
+    std::vector<SampleConfig> cfgs(N);
+    reinterpret_cast<GenState*>(state.data())->n_req = N;
+    RowState* rs = reinterpret_cast<RowState*>(state.data() + sizeof(GenState));
+    size_t off = 0;
+    for (int r = 0; r < N; ++r) {
+        const mb200_generate_params& gp = params[r];
+        const int P = prompt_off[r + 1] - prompt_off[r];
+        pre_off[r] = off;
+        for (int i = 0; i < nr; ++i) {      // prefill rows of the request: the negative prompt first (modeling_mapperatorinator.py:243-245)
+            const int64_t* src = (use_cfg && i == 0) ? neg_prompt : prompt;
+            for (int t = 0; t < P; ++t) pre[off + (size_t)i * P + t] = src[prompt_off[r] + t];
+        }
+        off += (size_t)nr * P;
+        for (int t = 0; t < P; ++t) idsrow[(size_t)r * ids_ld + t] = prompt[prompt_off[r] + t];
+        for (int i = 0; i < nr; ++i) { rowslot[r + i * N] = slots[r]; rowslot[m->max_rows + 2 * r + i] = slots[r]; }
+        rs[r].cur_len = P; rs[r].prompt_len = P; rs[r].max_length = gp.max_length; rs[r].min_new_tokens = gp.min_new_tokens;
+        for (int t = 0; t < ids_ld; ++t) if (t >= P) idsrow[(size_t)r * ids_ld + t] = gp.pad_token_id;
+        cfgs[r] = make_sample_config(&gp, N, use_cfg, V, ids_ld);
+        cfgs[r].pos_rule_cumsum = 0; cfgs[r].vflags_ld = Vin;
+    }
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_prefill_ids.p, pre.data(), pre.size() * 8, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_ids.p, idsrow.data(), idsrow.size() * 8, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->g_keyvalid.p, 1, (size_t)m->max_rows * ids_ld, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->g_leftpad.p, 0, m->max_rows * sizeof(int), st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_rowslot.p, rowslot.data(), rowslot.size() * 4, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_vflags.p, vflags, (size_t)N * Vin, cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_state.p, state.data(), state.size(), cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_cfg.p, cfgs.data(), cfgs.size() * sizeof(SampleConfig), cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->d_ticket.p, 0, (size_t)m->max_rows * c.heads * sizeof(int), st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));   // host vectors go out of scope; the copies above are from pageable memory
+
+    GenState* gs = m->g_state.as<GenState>();
+    MB_TRY(launch_prompt_scan_ragged(m->g_ids.as<long long>(), ids_ld, N, gs, m->g_vflags.as<unsigned char>(), Vin, cfgs[0].ts_start,
+                                     cfgs[0].ts_end, m->g_lastts.as<int>(), st));
+    // prefill of request r == the prefill of its batch-1 call, into cache rows r (and N + r); its last-position logits land in the
+    // logits rows of the same index, then ONE ragged selection picks every first token
+    for (int r = 0; r < N; ++r) {
+        const int P = prompt_off[r + 1] - prompt_off[r];
+        MB_TRY(decoder_prefill(m, nr, P, m->g_prefill_ids.as<long long>() + pre_off[r], 0, st, r, N, m->g_rowslot.as<int>() + m->max_rows + 2 * r));
+        GemvParams g = final_logits_params(m, nr, m->p_x.as<float>() + (size_t)(P - 1) * d, (long long)P * d);
+        g.seg[0].out += (size_t)r * V; g.seg[0].out_bs = (long long)N * V;
+        MB_TRY(launch_gemv(g, st, false));
+    }
+    MB_TRY(launch_sample(sample_params(m, rows), N, st, false, true));
+
+    // ---- token loop: one replay of the ragged step graph per token; its key never meets a uniform (.., 1) or beam (.., K) graph ----
+    auto key = std::make_tuple(rows, N, n_splits_grid, -1);
+    auto it = m->graphs.find(key);
+    if (it == m->graphs.end()) {
+        cudaGraph_t graph;
+        if (!m->cap_stream) MB_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
+        MB_CUDA_CHECK(cudaStreamSynchronize(st));
+        MB_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
+        const long long before = g_launch_count;
+        int s = token_step(m, rows, N, n_splits_grid, m->cap_stream, m->use_pdl, nullptr, nullptr, true);
+        cudaError_t e = cudaStreamEndCapture(m->cap_stream, &graph);
+        m->graph_nodes[key] = g_launch_count - before;
+        g_launch_count = before;
+        if (s) return s;
+        MB_CUDA_CHECK(e);
+        cudaGraphExec_t exec;
+        MB_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
+        cudaGraphDestroy(graph);
+        it = m->graphs.emplace(key, exec).first;
+    }
+    int produced = 1;
+    while (remaining > 0) {
+        int burst = std::min(remaining, 16);
+        if (first_poll > produced) burst = std::min(remaining, std::max(burst, first_poll - produced));
+        for (int i = 0; i < burst; ++i) MB_CUDA_CHECK(cudaGraphLaunch(it->second, st));
+        g_launch_count += (long long)burst * m->graph_nodes[key];
+        remaining -= burst; produced += burst;
+        MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag, &gs->all_finished, 4, cudaMemcpyDeviceToHost, st));
+        MB_CUDA_CHECK(cudaStreamSynchronize(st));
+        if (*m->h_flag) break;
+    }
+    MB_CUDA_CHECK(cudaMemcpyAsync(state.data(), m->g_state.p, state.size(), cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpy2DAsync(out_ids, (size_t)out_ld * 8, m->g_ids.p, (size_t)ids_ld * 8, (size_t)std::min((int)out_ld, ids_ld) * 8, N,
+                                    cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int r = 0; r < N; ++r) {
+        MB_REQUIRE(rs[r].finished && rs[r].cur_len <= params[r].max_length, "ragged token loop ended with an unfinished row");
+        out_len[r] = rs[r].cur_len;
+    }
     return 0;
 }
 

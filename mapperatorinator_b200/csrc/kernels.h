@@ -154,8 +154,28 @@ struct GenState {            // device-resident, one per engine
     int all_finished;
     int has_last_scores;
     int step;                // decode steps since the start of this call (RNG counter)
-    int pad_[7];
+    int n_req;               // ragged call: un-doubled rows of the call (0 in a uniform call)
+    int pad_[6];
 };
+
+// Ragged call (mb200_model_generate_ragged): every request is its own batch-1 call.  The GenState above keeps what the rows share
+// (all rows start together: step, has_last_scores, the tickets); what differs per row follows it IN THE SAME device buffer, so a
+// kernel that holds the GenState pointer finds row b's state at ragged_rows(st)[b].  Decoder row r (2B rows under CFG) belongs to
+// request r % B.
+struct RowState {
+    int cur_len;             // tokens in this row's ids (prompt + generated); its next token goes to ids[b][cur_len]
+    int prompt_len;
+    int max_length;
+    int min_new_tokens;
+    int finished;            // stopped on its own EOS set or max_length: the row appends nothing more, to its ids or to its cache
+    int pad_[3];
+};
+__host__ __device__ inline const RowState* ragged_rows(const GenState* st) { return reinterpret_cast<const RowState*>(st + 1); }
+__host__ __device__ inline RowState* ragged_rows(GenState* st) { return reinterpret_cast<RowState*>(st + 1); }
+
+// split-KV layout of the self-attention cache of ONE call: one 128-key split while the context fits, 64-key splits beyond.  A ragged
+// row keeps the plan of its own max_length, whatever its neighbours need: its partials and their merge order are its own call's.
+__host__ __device__ inline int self_splits(int max_length) { return max_length <= 128 ? 1 : (max_length + 63) / 64; }
 
 struct SampleConfig {        // device-resident, rewritten by the host once per generate() call
     int B;                   // un-doubled batch rows
@@ -174,6 +194,7 @@ struct SampleConfig {        // device-resident, rewritten by the host once per 
     int pad_id;
     int pos_rule_cumsum;     // 0: position = index (transformers 5.x), 1: index - n_left_pad[b] (4.5x)
     int ids_ld;              // row stride of the ids buffer
+    int vflags_ld;           // ragged call: one SampleConfig and one vocabulary-flag row per request, flags of request b at vflags + b * vflags_ld
 };
 
 enum XMode : int { X_PLAIN = 0, X_LAYERNORM = 1 };
@@ -197,7 +218,8 @@ struct GemvParams {
     const float* R; long long r_ld;                 // residual rows for segment 0 (null = none)
     const GenState* st;
 };
-int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl);
+// ragged: p.st heads a ragged state; segments with pos_stride write row b at ITS cache position, and not at all once it has finished
+int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged = false);
 
 struct DecAttnParams {
     const float* q; long long q_ld;                 // [rows, d_model], already scaled
@@ -215,6 +237,9 @@ struct DecAttnParams {
     const int* kv_src; long long kv_src_ld;         // beam search: [rows, kv_src_ld] cache row holding key position t of row r (null = row r)
 };
 int launch_decode_attention(const DecAttnParams& p, cudaStream_t stream, bool pdl);
+// Ragged self attention: p.st heads a ragged state; row r attends to its own cur_len keys with the split plan of its own max_length.
+// p.n_splits = splits of the grid (the largest plan of the call; also the row stride of the partials); p.chunk is not read.
+int launch_decode_attention_ragged(const DecAttnParams& p, cudaStream_t stream, bool pdl);
 
 struct SampleParams {
     const float* logits; long long logits_ld;       // [rows(2B if cfg), V]
@@ -238,7 +263,8 @@ struct SampleParams {
     int* ll_err;
     unsigned long long* trace;                      // tools/mega3_trace.py: clock64 stamps inside the selection phase (null in production)
 };
-int launch_sample(const SampleParams& p, int B, cudaStream_t stream, bool pdl);
+// ragged: cfg / vflags are per-request arrays, st heads a ragged state; row b runs the chain of its own batch-1 call
+int launch_sample(const SampleParams& p, int B, cudaStream_t stream, bool pdl, bool ragged = false);
 
 // ---- beam.cu: beam search (num_beams K <= 4) after the decoder's final logits ---------------------------------------------
 struct BeamParams {
@@ -339,6 +365,9 @@ int mega2_set_poll_sleep(int ns);                 // tuning: nanoseconds to back
 // one-time per call: scan the prompt for the MonotonicTimeShift state (logit_processors.py:149-166)
 int launch_prompt_scan(const long long* ids, long long ids_ld, int B, int P, const unsigned char* vflags, int ts_start, int ts_end,
                        int* last_ts, cudaStream_t stream);
+// the same per request of a ragged call: own prompt length (ragged state `st`) and own flag row
+int launch_prompt_scan_ragged(const long long* ids, long long ids_ld, int B, const GenState* st, const unsigned char* vflags, long long vflags_ld,
+                              int ts_start, int ts_end, int* last_ts, cudaStream_t stream);
 // prefill embedding: x[b, t] = tok_emb[ids[b, t]] + pos_emb[pos(b, t)]
 int launch_embed(const long long* ids, long long ids_ld, int rows, int B_ids, int P, const int* n_left_pad, int pos_rule_cumsum,
                  const float* tok_emb, const float* pos_emb, int d_model, float* x, cudaStream_t stream);

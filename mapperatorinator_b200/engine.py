@@ -187,6 +187,57 @@ class ModelEngine:
         L = out_len.value
         return torch.from_numpy(out.reshape(-1)[: B * L].reshape(B, L).copy())
 
+    def generate_ragged(self, requests: Sequence[tuple], layout: TokenLayout) -> List[torch.Tensor]:
+        """One token loop for independent requests `(slot, prompt ids (P_r,) without padding, generate_kwargs, negative prompt | None)`.
+        Requests may differ in prompt length, `max_length`, `min_new_tokens`, window kind (`lookback_time`, `lookahead_time`,
+        `context_type`), temperatures, `timeshift_bias`, sampling settings and `seed`, `cfg_scale`.  Returns one CPU LongTensor
+        (1, L_r) per request, equal to `generate([slot], prompt[None], None, layout, generate_kwargs, negative_prompt)` of that
+        request alone.  Classifier-free guidance is for every request of the call or for none; beam search has its own call."""
+        n = len(requests)
+        if n == 0:
+            return []
+        params = (_lib.GenerateParamsC * n)()
+        vflags = np.zeros((n, layout.vocab_size_in), dtype=np.uint8)
+        prompts, negs, cfg_rows = [], [], []
+        for r, (slot, prompt, gk, neg) in enumerate(requests):
+            if int(gk.get("num_beams", 1) or 1) != 1:
+                raise ValueError("a ragged call takes greedy or sampling requests; beam search (num_beams > 1) goes through generate()")
+            p, eos_ids, _ = self._generate_params(layout, gk)
+            ids = np.asarray(torch.as_tensor(prompt).detach().cpu().numpy(), dtype=np.int64).reshape(-1)
+            if not 1 <= ids.shape[0] < p.max_length <= self.cfg.tgt_seq_len:
+                raise ValueError(f"request {r}: need 1 <= prompt length ({ids.shape[0]}) < max_length ({p.max_length}) <= "
+                                 f"{self.cfg.tgt_seq_len}")
+            use_cfg = neg is not None and p.cfg_scale > 1.0
+            cfg_rows.append(use_cfg)
+            if not use_cfg:
+                p.cfg_scale = 1.0          # generate() runs such a request without guidance
+            neg_full = ids.copy()          # prepare_inputs_for_generation: the prompt with its first neg_len ids replaced
+            if use_cfg:
+                npn = np.asarray(torch.as_tensor(neg).detach().cpu().numpy(), dtype=np.int64).reshape(-1)
+                neg_full[:npn.shape[0]] = npn
+            params[r] = p
+            vflags[r] = build_vflags(layout, eos_ids)
+            prompts.append(ids); negs.append(neg_full)
+        if any(cfg_rows) and not all(cfg_rows):
+            raise ValueError("classifier-free guidance (negative prompt and cfg_scale > 1) on every request of a ragged call or on none")
+        rows = n * (2 if cfg_rows[0] else 1)
+        if rows > self.max_batch:
+            raise ValueError(f"{n} requests{' x 2 (classifier-free guidance)' if cfg_rows[0] else ''} = {rows} decoder rows; this engine "
+                             f"was built with max_batch={self.max_batch}")
+        off = np.zeros(n + 1, dtype=np.int32)
+        off[1:] = np.cumsum([len(x) for x in prompts])
+        flat = np.ascontiguousarray(np.concatenate(prompts))
+        nflat = np.ascontiguousarray(np.concatenate(negs)) if cfg_rows[0] else None
+        slots_a = np.ascontiguousarray(np.asarray([int(q[0]) for q in requests], dtype=np.int32))
+        ld = max(int(params[r].max_length) for r in range(n))
+        out = np.zeros((n, ld), dtype=np.int64)
+        out_len = np.zeros(n, dtype=np.int32)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.mb200_model_generate_ragged(
+                self.handle, n, slots_a.ctypes.data, flat.ctypes.data, off.ctypes.data, None if nflat is None else nflat.ctypes.data,
+                vflags.ctypes.data, C.cast(params, C.c_void_p), out.ctypes.data, ld, out_len.ctypes.data, _stream()))
+        return [torch.from_numpy(out[r, :out_len[r]].copy())[None] for r in range(n)]
+
     def generate_beams(self, slots: Sequence[int], prompt: torch.Tensor, prompt_mask: Optional[torch.Tensor], layout: TokenLayout,
                        generate_kwargs: dict, negative_prompt: Optional[torch.Tensor] = None,
                        negative_mask: Optional[torch.Tensor] = None, position_rule: str = "arange"):

@@ -99,6 +99,25 @@ class SongDecoder:
                 streams[s].append(ids[s, prompt.shape[1]:].tolist())
         return streams
 
+    def decode_songs_ragged(self, window_counts: Sequence[int], prompt_fn: Callable[[int, int, List[List[int]]], List[int]],
+                            generate_kwargs_fn: Callable[[int, int], dict], windows_per_song: Optional[int] = None
+                            ) -> List[List[List[int]]]:
+        """`decode_songs` for real prompts: song s has `window_counts[s]` windows (song s, window i at slot s * windows_per_song + i),
+        window i of every song that still has one is one row of a ragged `generate_ragged` call, so prompts may differ in length
+        (`prompt_fn(s, i, streams_of_song_s)`) and rows in kind (`generate_kwargs_fn(s, i)`: first and last windows of different songs
+        share a step).  A song drops out of the batch when it ends.  Each stream equals `decode_windows` run on that song alone.
+        Returns streams[s][i]."""
+        stride = windows_per_song or max(window_counts)
+        streams: List[List[List[int]]] = [[] for _ in window_counts]
+        for i in range(max(window_counts)):
+            live = [s for s, n in enumerate(window_counts) if i < n]
+            prompts = [prompt_fn(s, i, streams[s]) for s in live]
+            outs = self.engine.generate_ragged([(s * stride + i, torch.tensor(p, dtype=torch.long), generate_kwargs_fn(s, i), None)
+                                                for s, p in zip(live, prompts)], self.layout)
+            for s, p, ids in zip(live, prompts, outs):
+                streams[s].append(ids[0, len(p):].tolist())
+        return streams
+
 
 def trim_predicted_tokens(tokens: Sequence[int], layout: TokenLayout, context_type: Optional[str] = "map", lookback_ms: float = 0.0,
                           lookahead_max_ms: float = 0.0, trim_lookback: bool = False, trim_lookahead: bool = False,

@@ -57,6 +57,39 @@ def model_generate(model, tokenizer, model_kwargs, generate_kwargs):
 
 
 @torch.no_grad()
+def model_generate_requests(model, tokenizer, requests):
+    """Several independent `model_generate` calls of batch size 1 in ONE token loop (what `Processor.generate_sequential` issues one
+    after another, and what `InferenceServer._batch_thread` packs from several clients).  `requests` is a list of
+    `(model_kwargs, generate_kwargs)` with batch-1 tensors and no padding; the result is a list of `(ids, stats)` equal, request by
+    request, to `model_generate(model, tokenizer, model_kwargs, generate_kwargs)`; `elapsed_seconds` is the shared call's."""
+    layout = TokenLayout.from_tokenizer(tokenizer)
+    n = len(requests)
+    if n > model.engine.max_windows:
+        raise ValueError(f"{n} requests need {n} encoder slots; this engine was built with max_windows={model.engine.max_windows}")
+    reqs = []
+    for r, (mk, gk) in enumerate(requests):
+        gk = dict(gk)
+        gk.pop("precision", None)
+        ids = mk["decoder_input_ids"]
+        if ids.shape[0] != 1 or mk["inputs"].shape[0] != 1:
+            raise ValueError("every request of a ragged call is a batch-1 call")
+        mask = mk.get("decoder_attention_mask")
+        if isinstance(mask, torch.Tensor) and not bool(mask.all()):
+            raise ValueError("a request of a ragged call carries its prompt without padding")
+        neg = mk.get("negative_prompt")
+        reqs.append((r, ids[0], gk, None if neg is None else neg[0]))
+    start = time.perf_counter()
+    model.engine.encode(torch.cat([mk["inputs"] for mk, _ in requests]).to(model.device, torch.float32), slot_begin=0)
+    results = model.engine.generate_ragged(reqs, layout)
+    elapsed = time.perf_counter() - start
+    out = []
+    for (mk, gk), res in zip(requests, results):
+        pad_token_id = gk.get("pad_token_id", getattr(tokenizer, "pad_id", None))
+        out.append((res, _build_generation_stats(res, mk, pad_token_id, elapsed)))
+    return out
+
+
+@torch.no_grad()
 def model_forward(model, model_kwargs, generate_kwargs):
     """server.py:159-181 (cfg_scale == 1 path): teacher-forced fp32 logits on the CPU."""
     out = model.forward(frames=model_kwargs["inputs"], decoder_input_ids=model_kwargs["decoder_input_ids"],
