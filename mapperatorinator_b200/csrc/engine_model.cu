@@ -3,6 +3,7 @@
 // (osuT5/osuT5/inference/server.py:83-156) — see include/mapperatorinator_b200.h for the boundary.
 #include <algorithm>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <tuple>
 #include <unordered_map>
@@ -65,6 +66,9 @@ struct mb200_model {
     DevBuf d_attn, d_ticket;            // merged attention heads [rows, d] and the per-(row, head) arrival counters of the split merge
     DevBuf g_state, g_cfg, g_vflags, g_ids, g_prefill_ids, g_keyvalid, g_leftpad, g_rowslot, g_finished, g_lastts, g_lastscores;
     int* h_flag = nullptr;              // pinned
+    unsigned char* h_stage = nullptr;   // pinned staging of a generate call's state (prompt ids, masks, slots, flags, GenState, SampleConfig)
+    size_t h_stage_bytes = 0;
+    cudaEvent_t stage_ev = nullptr;     // recorded behind the staging copies: h_stage may be refilled once it has completed
     // graph keys carry B as well as rows: the captured sample kernel's grid is dim3(B), and a CFG call (B = 1, rows = 2) must
     // never replay the graph of a plain batch-2 call (B = 2, rows = 2)
     // ... and the beam count: a beam call ends its token step in the beam kernels and must never replay a greedy graph of equal rows
@@ -192,6 +196,8 @@ extern "C" void mb200_model_destroy(mb200_model* m) {
     if (m->cap_stream) cudaStreamDestroy(m->cap_stream);
     mel_plan_destroy(m->mel);
     if (m->h_flag) cudaFreeHost(m->h_flag);
+    if (m->h_stage) cudaFreeHost(m->h_stage);
+    if (m->stage_ev) cudaEventDestroy(m->stage_ev);
     delete m;
 }
 
@@ -336,6 +342,12 @@ extern "C" int mb200_model_finalize(mb200_model* m) {
     MB_TRY(m->g_leftpad.ensure(m->max_rows * sizeof(int)));
     MB_TRY(m->g_rowslot.ensure((size_t)3 * m->max_rows * sizeof(int)));   // [max_rows] decode rows, then one (slot, slot) pair per request for ragged prefills
     MB_TRY(m->g_finished.ensure(m->max_rows));
+    {
+        const size_t tgt = (size_t)m->max_rows * c.tgt_seq_len;
+        m->h_stage_bytes = tgt * 8 * 2 + tgt + (size_t)2 * m->max_rows * 4 + c.vocab_size_in + sizeof(GenState) + sizeof(SampleConfig) + 8 * 16;
+        MB_CUDA_CHECK(cudaMallocHost(&m->h_stage, m->h_stage_bytes));
+        MB_CUDA_CHECK(cudaEventCreateWithFlags(&m->stage_ev, cudaEventDisableTiming));
+    }
     MB_TRY(m->g_lastts.ensure(m->max_rows * sizeof(int)));
     MB_TRY(m->g_lastscores.ensure((size_t)2 * m->max_rows * c.vocab_size_out * sizeof(float)));
     MB_TRY(m->d_x.ensure((size_t)m->max_rows * d * sizeof(float)));
@@ -724,7 +736,9 @@ static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaSt
 }
 
 // The persistent path: all remaining tokens of the call in one cooperative launch (rows <= 2, weight slices must fit).
-static int run_megakernel(mb200_model* m, int rows, int B, int n_splits_self, int max_steps, cudaStream_t st) {
+// `before_sync` enqueues the caller's read-backs ahead of the launch's closing sync, so the call needs only that one host wait.
+static int run_megakernel(mb200_model* m, int rows, int B, int n_splits_self, int max_steps, cudaStream_t st,
+                          const std::function<int()>& before_sync) {
     auto key = std::make_pair(rows, n_splits_self);
     auto it = m->mega_phases.find(key);
     if (it == m->mega_phases.end()) {
@@ -750,6 +764,7 @@ static int run_megakernel(mb200_model* m, int rows, int B, int n_splits_self, in
     MB_CUDA_CHECK(cudaEventRecord(m->mega_ev[1], st));
     MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 1, m->g_megasync.as<int>() + 8, 4, cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 3, &m->g_state.as<GenState>()->cur_len, 4, cudaMemcpyDeviceToHost, st));
+    MB_TRY(before_sync());
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
     {
         float ms = 0.f;
@@ -761,7 +776,8 @@ static int run_megakernel(mb200_model* m, int rows, int B, int n_splits_self, in
 }
 
 // The dataflow path: same phase list, each phase annotated with the exchange buffers it reads / writes.
-static int run_megakernel2(mb200_model* m, int rows, int B, int n_splits_self, int max_steps, cudaStream_t st) {
+static int run_megakernel2(mb200_model* m, int rows, int B, int n_splits_self, int max_steps, cudaStream_t st,
+                           const std::function<int()>& before_sync) {
     auto key = std::make_tuple(rows, B, n_splits_self);
     auto it = m->mega2_phases.find(key);
     if (it == m->mega2_phases.end()) {
@@ -826,6 +842,7 @@ static int run_megakernel2(mb200_model* m, int rows, int B, int n_splits_self, i
     MB_CUDA_CHECK(cudaEventRecord(m->mega_ev[1], st));
     MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 1, m->g_megasync.as<int>() + 8, 4, cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 3, &m->g_state.as<GenState>()->cur_len, 4, cudaMemcpyDeviceToHost, st));
+    MB_TRY(before_sync());
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
     {
         float ms = 0.f;
@@ -904,17 +921,30 @@ extern "C" int mb200_model_generate(mb200_model* m, const int32_t* slots, int32_
     gs.cur_len = P; gs.prompt_len = P; gs.max_length = gp->max_length; gs.min_new_tokens = gp->min_new_tokens;
     const SampleConfig sc = make_sample_config(gp, B, use_cfg, V, ids_ld);
 
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_prefill_ids.p, pre.data(), pre.size() * 8, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_ids.p, idsrow.data(), idsrow.size() * 8, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_keyvalid.p, kv.data(), kv.size(), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_leftpad.p, leftpad.data(), rows * 4, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_rowslot.p, rowslot.data(), rows * 4, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_vflags.p, vflags, c.vocab_size_in, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_state.p, &gs, sizeof(gs), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_cfg.p, &sc, sizeof(sc), cudaMemcpyHostToDevice, st));
+    // The call state leaves from the engine's pinned staging buffer, so the copies are asynchronous and the prefill queues behind them
+    // with no host wait.  The buffer is refilled only once the previous call's copies completed (that call's closing sync normally
+    // saw to it; the event covers a call that returned early on an error).
+    MB_CUDA_CHECK(cudaEventSynchronize(m->stage_ev));
+    size_t stage_off = 0;
+    auto stage = [&](void* dst, const void* src, size_t n) -> int {
+        stage_off = (stage_off + 15) & ~size_t(15);
+        MB_REQUIRE(stage_off + n <= m->h_stage_bytes, "call state exceeds the staging buffer");
+        std::memcpy(m->h_stage + stage_off, src, n);
+        MB_CUDA_CHECK(cudaMemcpyAsync(dst, m->h_stage + stage_off, n, cudaMemcpyHostToDevice, st));
+        stage_off += n;
+        return 0;
+    };
+    MB_TRY(stage(m->g_prefill_ids.p, pre.data(), pre.size() * 8));
+    MB_TRY(stage(m->g_ids.p, idsrow.data(), idsrow.size() * 8));
+    MB_TRY(stage(m->g_keyvalid.p, kv.data(), kv.size()));
+    MB_TRY(stage(m->g_leftpad.p, leftpad.data(), rows * 4));
+    MB_TRY(stage(m->g_rowslot.p, rowslot.data(), rows * 4));
+    MB_TRY(stage(m->g_vflags.p, vflags, c.vocab_size_in));
+    MB_TRY(stage(m->g_state.p, &gs, sizeof(gs)));
+    MB_TRY(stage(m->g_cfg.p, &sc, sizeof(sc)));
+    MB_CUDA_CHECK(cudaEventRecord(m->stage_ev, st));
     MB_CUDA_CHECK(cudaMemsetAsync(m->g_finished.p, 0, m->max_rows, st));
     MB_CUDA_CHECK(cudaMemsetAsync(m->d_ticket.p, 0, (size_t)m->max_rows * m->cfg.heads * sizeof(int), st));   // self-resetting; cleared in case a previous call aborted
-    MB_CUDA_CHECK(cudaStreamSynchronize(st));   // host vectors go out of scope; the copies above are from pageable memory
 
     // partial buffers for the split-KV attentions
     const int chunk = 64;
@@ -977,13 +1007,22 @@ extern "C" int mb200_model_generate(mb200_model* m, const int32_t* slots, int32_
         }
         // (one 256-key attention unit per head for contexts of 129..256 tokens was tried: 365 vs 344 us / token against three 64-key units +
         //  merge — the V rows beyond the first 64 keys are fetched inside the PV loop, and the wider unit costs instructions in EVERY unit)
-        if (dataflow) MB_TRY(run_megakernel2(m, rows, B, n_splits_self, gp->max_length - (P + 1), st));
-        else MB_TRY(run_megakernel(m, rows, B, n_splits_self, gp->max_length - (P + 1), st));
-        MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag, &m->g_state.as<GenState>()->cur_len, 4, cudaMemcpyDeviceToHost, st));
-        MB_CUDA_CHECK(cudaStreamSynchronize(st));
-        const int Lm = *m->h_flag;
-        MB_CUDA_CHECK(cudaMemcpy2DAsync(out_ids, (size_t)Lm * 8, m->g_ids.p, (size_t)ids_ld * 8, (size_t)Lm * 8, B, cudaMemcpyDeviceToHost, st));
-        MB_CUDA_CHECK(cudaStreamSynchronize(st));
+        // every row's ids up to max_length come back with {error flag, cur_len} ahead of the one sync; the final length is known only
+        // then, so the rows are packed into out_ids ([B, cur_len]) on the host.  The staging copies of this call completed before the
+        // megakernel started (stream order), so the pinned staging buffer is free to receive them.
+        const int Lmax = gp->max_length;
+        MB_REQUIRE((size_t)B * Lmax * 8 <= m->h_stage_bytes, "ids exceed the staging buffer");
+        long long* ids_back = reinterpret_cast<long long*>(m->h_stage);
+        auto read_ids = [&]() -> int {
+            MB_CUDA_CHECK(cudaMemcpy2DAsync(ids_back, (size_t)Lmax * 8, m->g_ids.p, (size_t)ids_ld * 8, (size_t)Lmax * 8, B,
+                                            cudaMemcpyDeviceToHost, st));
+            return 0;
+        };
+        if (dataflow) MB_TRY(run_megakernel2(m, rows, B, n_splits_self, gp->max_length - (P + 1), st, read_ids));
+        else MB_TRY(run_megakernel(m, rows, B, n_splits_self, gp->max_length - (P + 1), st, read_ids));
+        const int Lm = m->h_flag[3];      // cur_len after the launch
+        MB_REQUIRE(Lm >= P + 1 && Lm <= Lmax, "megakernel left an out-of-range length");
+        for (int b = 0; b < B; ++b) std::memcpy(out_ids + (size_t)b * Lm, ids_back + (size_t)b * Lmax, (size_t)Lm * 8);
         *out_len = Lm;
         return 0;
     }

@@ -16,13 +16,17 @@ namespace {
 
 constexpr int BM = 128, BN = 128, BK = 16, PAD = 4;
 
+// MH 64-row halves per tile: 2 = the 128x128 tile, 1 = a 64x128 tile for launches of at most one 128-row tile, whose padding rows
+// would otherwise cost as many FMAs as the real ones.  Each output's sum runs over the same k in the same order either way.
+template <int MH>
 __global__ void __launch_bounds__(256, 2) gemm_f32_kernel(GemmParams p) {
-    __shared__ __align__(16) float As[2][BK][BM + PAD];
+    constexpr int TM = 64 * MH;
+    __shared__ __align__(16) float As[2][BK][TM + PAD];
     __shared__ __align__(16) float Bs[2][BK][BN + PAD];
 
     const int tid = threadIdx.x;
     const int tx = tid & 15, ty = tid >> 4;
-    const long long m0 = (long long)blockIdx.y * BM;
+    const long long m0 = (long long)blockIdx.y * TM;
     const int n0 = blockIdx.x * BN;
 
     // global->smem loader coordinates: two rows per operand per thread, one float4 along K each
@@ -34,16 +38,16 @@ __global__ void __launch_bounds__(256, 2) gemm_f32_kernel(GemmParams p) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         long long m = m0 + lrow + h * 64;
-        a_ok[h] = m < p.M;
+        a_ok[h] = h < MH && m < p.M;
         a_ptr[h] = a_ok[h] ? p.A.row(p.m_base + m) : p.A.ptr;
         int n = n0 + lrow + h * 64;
         w_ok[h] = n < p.N;
         w_ptr[h] = p.W + (long long)(w_ok[h] ? n : 0) * p.ldw;
     }
 
-    float acc[8][8];
+    float acc[4 * MH][8];
 #pragma unroll
-    for (int i = 0; i < 8; ++i)
+    for (int i = 0; i < 4 * MH; ++i)
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
 
@@ -54,7 +58,7 @@ __global__ void __launch_bounds__(256, 2) gemm_f32_kernel(GemmParams p) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             int k = k_lo_ + k0 + lk;
-            ra[h] = (a_ok[h] && k < k_hi_) ? __ldg(reinterpret_cast<const float4*>(a_ptr[h] + k)) : make_float4(0, 0, 0, 0);
+            if (h < MH) ra[h] = (a_ok[h] && k < k_hi_) ? __ldg(reinterpret_cast<const float4*>(a_ptr[h] + k)) : make_float4(0, 0, 0, 0);
             rw[h] = (w_ok[h] && k < k_hi_) ? __ldg(reinterpret_cast<const float4*>(w_ptr[h] + k)) : make_float4(0, 0, 0, 0);
         }
     };
@@ -62,7 +66,7 @@ __global__ void __launch_bounds__(256, 2) gemm_f32_kernel(GemmParams p) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             int r = lrow + h * 64;
-            As[buf][lk + 0][r] = ra[h].x; As[buf][lk + 1][r] = ra[h].y; As[buf][lk + 2][r] = ra[h].z; As[buf][lk + 3][r] = ra[h].w;
+            if (h < MH) { As[buf][lk + 0][r] = ra[h].x; As[buf][lk + 1][r] = ra[h].y; As[buf][lk + 2][r] = ra[h].z; As[buf][lk + 3][r] = ra[h].w; }
             Bs[buf][lk + 0][r] = rw[h].x; Bs[buf][lk + 1][r] = rw[h].y; Bs[buf][lk + 2][r] = rw[h].z; Bs[buf][lk + 3][r] = rw[h].w;
         }
     };
@@ -79,13 +83,13 @@ __global__ void __launch_bounds__(256, 2) gemm_f32_kernel(GemmParams p) {
 #pragma unroll
         for (int k = 0; k < BK; ++k) {
             float4 a0 = *reinterpret_cast<const float4*>(&As[buf][k][ty * 4]);
-            float4 a1 = *reinterpret_cast<const float4*>(&As[buf][k][64 + ty * 4]);
+            float4 a1 = MH == 2 ? *reinterpret_cast<const float4*>(&As[buf][k][64 * (MH - 1) + ty * 4]) : a0;
             float4 b0 = *reinterpret_cast<const float4*>(&Bs[buf][k][tx * 4]);
             float4 b1 = *reinterpret_cast<const float4*>(&Bs[buf][k][64 + tx * 4]);
             float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
             float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
-            for (int i = 0; i < 8; ++i)
+            for (int i = 0; i < 4 * MH; ++i)
 #pragma unroll
                 for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
         }
@@ -98,7 +102,7 @@ __global__ void __launch_bounds__(256, 2) gemm_f32_kernel(GemmParams p) {
     // ---- epilogue --------------------------------------------------------------------------------------------------
     if (p.splitk > 1) {      // raw partial sums; gemm_splitk_reduce_kernel finishes the job
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
+        for (int i = 0; i < 4 * MH; ++i) {
             long long m = m0 + (i < 4 ? ty * 4 + i : 64 + ty * 4 + (i - 4));
             if (m >= p.M) continue;
             float* wrow = p.splitk_ws + ((long long)blockIdx.z * p.M + m) * p.N;
@@ -113,7 +117,7 @@ __global__ void __launch_bounds__(256, 2) gemm_f32_kernel(GemmParams p) {
         return;
     }
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
+    for (int i = 0; i < 4 * MH; ++i) {
         long long m = m0 + (i < 4 ? ty * 4 + i : 64 + ty * 4 + (i - 4));
         if (m >= p.M) continue;
         float* crow = p.C.row(p.m_base + m);
@@ -230,9 +234,12 @@ int launch_gemm(const GemmParams& p, cudaStream_t stream, GemmCtx* ctx) {
     int kps = 0;
     const int splits = gemm_splits_simt(p.N, p.K, ctx->num_sms, &kps);
     const int tiles_n = (p.N + BN - 1) / BN;
+    const bool half = p.M <= BM;      // one row tile: 64-row tiles halve the padded FMAs (and double the CTAs when M > 64)
+    const int tm = half ? BM / 2 : BM;
     if (splits == 1) {
-        dim3 grid(tiles_n, (unsigned)((p.M + BM - 1) / BM));
-        gemm_f32_kernel<<<grid, 256, 0, stream>>>(p);
+        dim3 grid(tiles_n, (unsigned)((p.M + tm - 1) / tm));
+        if (half) gemm_f32_kernel<1><<<grid, 256, 0, stream>>>(p);
+        else gemm_f32_kernel<2><<<grid, 256, 0, stream>>>(p);
         MB_LAUNCH_CHECK();
         ++g_launch_count;
         return 0;
@@ -250,7 +257,9 @@ int launch_gemm(const GemmParams& p, cudaStream_t stream, GemmCtx* ctx) {
         q.m_base = p.m_base + m0;
         q.M = (int)std::min<long long>(rows_per_pass, p.M - m0);
         q.splitk_ws = ctx->splitk_ws; q.splitk = splits; q.k_per_split = kps; q.split_mode = 1;
-        gemm_f32_kernel<<<dim3(tiles_n, (unsigned)((q.M + BM - 1) / BM), splits), 256, 0, stream>>>(q);
+        const dim3 grid(tiles_n, (unsigned)((q.M + tm - 1) / tm), splits);
+        if (half) gemm_f32_kernel<1><<<grid, 256, 0, stream>>>(q);
+        else gemm_f32_kernel<2><<<grid, 256, 0, stream>>>(q);
         MB_LAUNCH_CHECK();
         ++g_launch_count;
         const int s = launch_splitk_reduce(q, stream);

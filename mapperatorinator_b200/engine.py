@@ -62,6 +62,25 @@ def build_vflags(layout: TokenLayout, eos_ids: Sequence[int]) -> np.ndarray:
     return f
 
 
+class _VflagsCache:
+    """`build_vflags` per (layout, EOS set): sequential windows ask for the same few rows on every call.  Rows are read-only.
+    A layout is keyed by identity, so it must not be changed in place once an engine has generated with it (build a new one)."""
+
+    def __init__(self):
+        self._rows: Dict[tuple, tuple] = {}
+
+    def get(self, layout: TokenLayout, eos_ids: Sequence[int]) -> np.ndarray:
+        key = (id(layout), tuple(eos_ids))
+        hit = self._rows.get(key)
+        if hit is None or hit[0] is not layout:       # the layout object is held, so its id cannot be reused while cached
+            if len(self._rows) >= 64:
+                self._rows.clear()
+            f = build_vflags(layout, eos_ids)
+            f.setflags(write=False)
+            hit = self._rows[key] = (layout, f)
+        return hit[1]
+
+
 class ModelEngine:
     """Stage (ii): weights + resident encoder slots + KV arena behind `mb200_model_*`."""
 
@@ -73,6 +92,7 @@ class ModelEngine:
         self.device = torch.device(device)
         self.lib = _lib.load()
         self.max_windows, self.max_batch = max_windows, max_batch
+        self._vflags = _VflagsCache()
         basis = np.ascontiguousarray(mel_filterbank(cfg.mel) if mel_basis is None else mel_basis, dtype=np.float32)
         cc = _lib.ModelConfigC(cfg.d_model, cfg.encoder_layers, cfg.decoder_layers, cfg.heads, cfg.ffn_dim, cfg.src_seq_len,
                                cfg.tgt_seq_len, cfg.vocab_size_in, cfg.vocab_size_out, _mel_c(cfg.mel), max_windows, max_batch)
@@ -174,7 +194,7 @@ class ModelEngine:
             # the reference's negative_prompt_attention_mask is swallowed by HF generate()'s own parameter of that name
             # (transformers generation/utils.py:2142): the negative rows run with the conditional prompt's mask.
             nmsk = np.ascontiguousarray(msk.copy() if msk is not None else np.ones_like(ids, dtype=np.uint8))
-        vflags = build_vflags(layout, eos_ids)
+        vflags = self._vflags.get(layout, eos_ids)
         slots_a = np.ascontiguousarray(np.asarray(list(slots), dtype=np.int32))
         assert slots_a.shape[0] == B
         out = np.zeros((B, p.max_length), dtype=np.int64)
@@ -216,7 +236,7 @@ class ModelEngine:
                 npn = np.asarray(torch.as_tensor(neg).detach().cpu().numpy(), dtype=np.int64).reshape(-1)
                 neg_full[:npn.shape[0]] = npn
             params[r] = p
-            vflags[r] = build_vflags(layout, eos_ids)
+            vflags[r] = self._vflags.get(layout, eos_ids)
             prompts.append(ids); negs.append(neg_full)
         if any(cfg_rows) and not all(cfg_rows):
             raise ValueError("classifier-free guidance (negative prompt and cfg_scale > 1) on every request of a ragged call or on none")
@@ -270,7 +290,7 @@ class ModelEngine:
             neg_full[:, :npn.shape[1]] = npn
             neg = np.ascontiguousarray(neg_full)
             nmsk = np.ascontiguousarray(msk.copy() if msk is not None else np.ones_like(ids, dtype=np.uint8))
-        vflags = build_vflags(layout, eos_ids)
+        vflags = self._vflags.get(layout, eos_ids)
         slots_a = np.ascontiguousarray(np.asarray(list(slots), dtype=np.int32))
         assert slots_a.shape[0] == B
         fill = p.pad_token_id if p.pad_token_id else eos_ids[0]          # HF: `pad_token_id or eos_token_id[0]`
@@ -292,7 +312,7 @@ class ModelEngine:
         p, eos_ids, gk = self._generate_params(layout, generate_kwargs)
         B, L = ids.shape
         a = np.ascontiguousarray(ids.detach().cpu().numpy().astype(np.int64))
-        vflags = build_vflags(layout, eos_ids)
+        vflags = self._vflags.get(layout, eos_ids)
         logits = logits.contiguous().float()
         scores = torch.empty(B, self.cfg.vocab_size_out, device=logits.device, dtype=torch.float32)
         chosen = np.zeros(B, dtype=np.int64)
@@ -313,7 +333,7 @@ class ModelEngine:
         B = BK // num_beams
         a = np.ascontiguousarray(ids.detach().cpu().numpy().astype(np.int64))
         rs = np.ascontiguousarray(run_scores.detach().cpu().numpy().astype(np.float32))
-        vflags = build_vflags(layout, eos_ids)
+        vflags = self._vflags.get(layout, eos_ids)
         logits = logits.contiguous().float()
         lp = torch.empty(BK, self.cfg.vocab_size_out, device=logits.device, dtype=torch.float32)
         out = dict(top=np.zeros(BK, np.int32), parent=np.zeros(BK, np.int32), token=np.zeros(BK, np.int64), score=np.zeros(BK, np.float32),
