@@ -144,6 +144,18 @@ int mb200_model_generate_ragged(mb200_model* m, int32_t n_req, const int32_t* sl
 int mb200_model_forward_logits(mb200_model* m, const int32_t* slots, int32_t batch, const int64_t* ids, const uint8_t* mask,
                                int32_t len, int32_t position_rule, float* logits_out, void* cuda_stream);
 
+/* Per-token scores of the same teacher-forced pass (MaiMod's Processor.ai_mod, processor.py:519-525), without ever holding the
+ * call's [batch, len, vocab_size_out] logits: the projection runs in row chunks, each reduced on the device.  Same inputs as
+ * mb200_model_forward_logits.  Outputs: DEVICE [batch, len], indexed by the scored token j; for j >= 1, with
+ * p = softmax(logits[b, j - 1]) and y = ids[b, j]:
+ *   entropy   = -sum p log2(p + 1e-10);   surprisal = -log2(p_y + 1e-10);   relative = entropy > 0 ? surprisal / entropy : 0;
+ *   suggested = argmax logits[b, j - 1] (lowest index among ties).
+ * Column 0 is NaN (suggested -1); a target y >= vocab_size_out has NaN surprisal and relative.  The logits behind the scores are
+ * bit-identical to mb200_model_forward_logits' output for the same call. */
+int mb200_model_score_tokens(mb200_model* m, const int32_t* slots, int32_t batch, const int64_t* ids, const uint8_t* mask, int32_t len,
+                             int32_t position_rule, float* entropy, float* surprisal, float* relative, int64_t* suggested,
+                             void* cuda_stream);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Stage (iii): DiT + sampling loop.  Replaces DiT.forward_with_cfg (osu_diffusion/utils/models.py:301-317) and
  * SpacedDiffusion.p_sample_loop as called by DiffisionPipeline.sample_part (diffusion_pipeline.py:243-252).

@@ -51,6 +51,7 @@ ABI_SYMBOLS = [
     "mb200_mel_create", "mb200_mel_destroy", "mb200_mel_forward",
     "mb200_model_create", "mb200_model_destroy", "mb200_model_set_weight", "mb200_model_finalize", "mb200_model_encode",
     "mb200_model_generate", "mb200_model_generate_beams", "mb200_model_generate_ragged", "mb200_model_forward_logits",
+    "mb200_model_score_tokens",
     "mb200_dit_create", "mb200_dit_destroy", "mb200_dit_set_weight", "mb200_dit_finalize", "mb200_dit_forward_with_cfg",
     "mb200_dit_sample_loop", "mb200_dit_set_option", "mb200_dit_set_sliders", "mb200_dit_apply_sliders",
     "mb200_launch_count", "mb200_model_set_option", "mb200_model_profile_step", "mb200_model_read_trace", "mb200_model_mega_stats", "mb200_model_logits_chain",
@@ -86,6 +87,7 @@ def load() -> C.CDLL:
                                                C.POINTER(i32), vp, vp]
     lib.mb200_model_generate_ragged.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, i32, vp, vp]
     lib.mb200_model_forward_logits.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, vp]
+    lib.mb200_model_score_tokens.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, vp, vp, vp, vp]
     lib.mb200_model_set_option.argtypes = [vp, C.c_char_p, i32]
     lib.mb200_launch_count.restype = i64
     lib.mb200_model_profile_step.argtypes = [vp, i32, i32, i32, i32, vp, vp]

@@ -8,7 +8,7 @@ FLAGS=(-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 --expt-rel
 if [[ "${MB200_PTXAS_V:-0}" == "1" ]]; then FLAGS+=(-Xptxas -v); fi
 mkdir -p "${HERE}/build"
 pids=()
-for f in c_abi gemm gemm_tc norm attention attention_tc mel audio decode beam decode_mega decode_mega2 engine_model engine_dit slider; do
+for f in c_abi gemm gemm_tc norm attention attention_tc mel audio decode beam decode_mega decode_mega2 engine_model engine_dit slider score; do
   ( "${NVCC}" "${FLAGS[@]}" -c "${HERE}/${f}.cu" -o "${HERE}/build/${f}.o" ) &
   pids+=($!)
 done

@@ -101,6 +101,7 @@ struct mb200_model {
     DevBuf b_dbg;                       // beam-step parity hook outputs
     AttnCtx attn;                       // tensor-core attention scratch of the encoder (head-major tf32 copies of q | k | v^T)
     GemmCtx gemm;                       // this engine's GEMM scratch: split-K planes, tf32 activation copies, weight mirrors, error flag
+    DevBuf s_logits;                    // token scoring: one chunk of vocabulary-projection rows [<= SCORE_CHUNK_ROWS, V]
 
     int d() const { return cfg.d_model; }
     int Ts() const { return cfg.src_seq_len / 2; }
@@ -1368,12 +1369,13 @@ extern "C" int mb200_model_generate_beams(mb200_model* m, const int32_t* slots, 
     return 0;
 }
 
-extern "C" int mb200_model_forward_logits(mb200_model* m, const int32_t* slots, int32_t B, const int64_t* ids, const uint8_t* mask,
-                                          int32_t len, int32_t position_rule, float* logits_out, void* stream) {
+// Teacher-forced pass up to the final LayerNorm: stages ids / key mask / left padding / slots, runs the decoder prefill and leaves
+// the normalised hidden states of all B * len positions in p_h (what the vocabulary projection reads).
+static int teacher_forced_hidden(mb200_model* m, const int32_t* slots, int32_t B, const int64_t* ids, const uint8_t* mask, int32_t len,
+                                 int32_t position_rule, cudaStream_t st) {
     MB_REQUIRE(m && m->finalized, "model not finalized");
     MB_REQUIRE(B >= 1 && B <= m->max_rows && len >= 1 && len <= m->cfg.tgt_seq_len, "bad batch / length");
     const auto& c = m->cfg;
-    cudaStream_t st = (cudaStream_t)stream;
     const int ids_ld = c.tgt_seq_len, d = c.d_model;
     std::vector<unsigned char> kv((size_t)B * ids_ld, 1);
     std::vector<int> leftpad(B, 0), rowslot(B);
@@ -1396,10 +1398,50 @@ extern "C" int mb200_model_forward_logits(mb200_model* m, const int32_t* slots, 
     MB_CUDA_CHECK(cudaMemcpyAsync(m->g_rowslot.p, rowslot.data(), B * 4, cudaMemcpyHostToDevice, st));
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
     MB_TRY(decoder_prefill(m, B, len, m->g_prefill_ids.as<long long>(), position_rule, st));
+    MB_TRY(layernorm(m->p_x.as<float>(), m->p_h.as<float>(), m->dec_ln_w, m->dec_ln_b, B * len, d, 1e-5f, st));
+    return 0;
+}
+
+extern "C" int mb200_model_forward_logits(mb200_model* m, const int32_t* slots, int32_t B, const int64_t* ids, const uint8_t* mask,
+                                          int32_t len, int32_t position_rule, float* logits_out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    MB_TRY(teacher_forced_hidden(m, slots, B, ids, mask, len, position_rule, st));
+    const auto& c = m->cfg;
+    const int d = c.d_model;
     const int R = B * len;
-    MB_TRY(layernorm(m->p_x.as<float>(), m->p_h.as<float>(), m->dec_ln_w, m->dec_ln_b, R, d, 1e-5f, st));
     MB_TRY(launch_gemm(gemm_base(plain_map(m->p_h.as<float>(), d), m->proj_out, d, plain_map(logits_out, c.vocab_size_out), nullptr, R,
                                  c.vocab_size_out, d), st, &m->gemm));
+    return 0;
+}
+
+// Rows of one projection chunk in mb200_model_score_tokens.  >= 512 so that every chunk of a call of more rows is a tensor-core GEMM,
+// as the unchunked projection of forward_logits is; not a divisor of the usual B * L (powers of two), so the tests meet the overlapping
+// last chunk.
+static constexpr int SCORE_CHUNK_ROWS = 3072;
+
+extern "C" int mb200_model_score_tokens(mb200_model* m, const int32_t* slots, int32_t B, const int64_t* ids, const uint8_t* mask,
+                                        int32_t len, int32_t position_rule, float* entropy, float* surprisal, float* relative,
+                                        int64_t* suggested, void* stream) {
+    MB_REQUIRE(entropy && surprisal && relative && suggested, "null output");
+    cudaStream_t st = (cudaStream_t)stream;
+    MB_TRY(teacher_forced_hidden(m, slots, B, ids, mask, len, position_rule, st));
+    const auto& c = m->cfg;
+    const int d = c.d_model, V = c.vocab_size_out, R = B * len;
+    const int chunk = std::min(R, SCORE_CHUNK_ROWS);
+    MB_TRY(m->s_logits.ensure((size_t)chunk * V * sizeof(float)));
+    ScoreParams sp{};
+    sp.logits = m->s_logits.as<float>(); sp.ids = m->g_prefill_ids.as<long long>(); sp.L = len; sp.V = V;
+    sp.entropy = entropy; sp.surprisal = surprisal; sp.relative = relative; sp.suggested = reinterpret_cast<long long*>(suggested);
+    // Every chunk has the same M (the last one overlaps its predecessor instead of being short) and starts at m_base 0 of its own
+    // A pointer: tc_gemm_eligible sends m_base != 0 or M < 512 to the SIMT kernel, whose sums differ in the last bits, so this keeps
+    // each row on the GEMM path the single [R, V] projection of forward_logits takes, and every logit bit-identical to it.
+    for (int r0 = 0; r0 < R; r0 += chunk) {
+        const int row0 = std::min(r0, R - chunk);
+        MB_TRY(launch_gemm(gemm_base(plain_map(m->p_h.as<float>() + (size_t)row0 * d, d), m->proj_out, d, plain_map(m->s_logits.as<float>(), V),
+                                     nullptr, chunk, V, d), st, &m->gemm));
+        sp.row0 = row0;
+        MB_TRY(launch_score_rows(sp, chunk, st));
+    }
     return 0;
 }
 

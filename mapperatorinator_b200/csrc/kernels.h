@@ -132,6 +132,17 @@ void mel_plan_destroy(MelPlan* p);
 int launch_mel(const MelPlan* plan, const float* pcm, long long pcm_ld, int B, int n_samples, float* mel, long long mel_ld,
                long long mel_bs, cudaStream_t stream);
 
+// ---- score.cu: per-token statistics of a teacher-forced pass (processor.py:519-525) ------------------------------------
+struct ScoreParams {
+    const float* logits;           // [rows, V]: the projection rows row0 .. row0 + rows - 1 of the call
+    long long row0;                // global row (b * L + t) of logits row 0
+    const long long* ids;          // DEVICE [B * L] given ids (row r's target is ids[r + 1] when t + 1 < L)
+    int L, V;
+    float *entropy, *surprisal, *relative;   // DEVICE [B * L], indexed by the scored token
+    long long* suggested;
+};
+int launch_score_rows(const ScoreParams& p, int rows, cudaStream_t stream);
+
 }  // namespace mb200
 
 // =====================================================================================================================

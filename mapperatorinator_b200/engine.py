@@ -362,6 +362,46 @@ class ModelEngine:
                                                            {"arange": 0, "mask_cumsum": 1}[position_rule], out.data_ptr(), _stream()))
         return out
 
+    def _score_args(self, slots: Sequence[int], ids: torch.Tensor, mask: Optional[torch.Tensor]):
+        """Validates a scoring call on the host (ValueError before anything is launched) -> (ids, mask, slots) as numpy arrays."""
+        if ids.dim() != 2:
+            raise ValueError(f"ids must be [B, L], got shape {tuple(ids.shape)}")
+        B, L = ids.shape
+        slots = list(slots)
+        if len(slots) != B:
+            raise ValueError(f"{B} rows need {B} encoder slots, got {len(slots)}")
+        if not 1 <= B <= self.max_batch:
+            raise ValueError(f"{B} rows; this engine was built with max_batch={self.max_batch}")
+        if not 1 <= L <= self.cfg.tgt_seq_len:
+            raise ValueError(f"length {L} is outside 1..tgt_seq_len={self.cfg.tgt_seq_len}")
+        if any(not 0 <= s < self.max_windows for s in slots):
+            raise ValueError(f"encoder slots must lie in 0..{self.max_windows - 1}")
+        a = np.ascontiguousarray(ids.detach().cpu().numpy().astype(np.int64))
+        if a.min() < 0 or a.max() >= self.cfg.vocab_size_in:
+            raise ValueError(f"token ids must lie in 0..{self.cfg.vocab_size_in - 1}")
+        if mask is not None and tuple(mask.shape) != (B, L):
+            raise ValueError(f"mask shape {tuple(mask.shape)} differs from ids shape {(B, L)}")
+        m = None if mask is None else np.ascontiguousarray(mask.detach().cpu().numpy().astype(np.uint8))
+        return a, m, np.ascontiguousarray(np.asarray(slots, dtype=np.int32))
+
+    def score_tokens(self, slots: Sequence[int], ids: torch.Tensor, mask: Optional[torch.Tensor],
+                     position_rule: str = "arange") -> Dict[str, torch.Tensor]:
+        """Per-token scores of the teacher-forced pass `forward_logits` runs on the same arguments (MaiMod, processor.py:519-525),
+        without the [B, L, V] logits ever existing.  Returns device tensors [B, L] indexed by the scored token j: `entropy`,
+        `surprisal`, `relative` (float32; NaN in column 0, and in surprisal / relative where ids[b, j] >= vocab_size_out) and
+        `suggested` (int64 argmax of the logits row j - 1; -1 in column 0).  Every position is scored whatever the mask says."""
+        a, m, slots_a = self._score_args(slots, ids, mask)
+        B, L = a.shape
+        out = {k: torch.empty(B, L, device=self.device, dtype=torch.float32) for k in ("entropy", "surprisal", "relative")}
+        out["suggested"] = torch.empty(B, L, device=self.device, dtype=torch.int64)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.mb200_model_score_tokens(self.handle, slots_a.ctypes.data, B, a.ctypes.data,
+                                                         None if m is None else m.ctypes.data, L,
+                                                         {"arange": 0, "mask_cumsum": 1}[position_rule], out["entropy"].data_ptr(),
+                                                         out["surprisal"].data_ptr(), out["relative"].data_ptr(),
+                                                         out["suggested"].data_ptr(), _stream()))
+        return out
+
     def set_option(self, name: str, value: int) -> None:
         _lib.check(self.lib.mb200_model_set_option(self.handle, name.encode(), int(value)))
 

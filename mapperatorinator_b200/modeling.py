@@ -86,4 +86,17 @@ class B200Mapperatorinator:
         logits = self.engine.forward_logits(list(range(B)), decoder_input_ids, decoder_attention_mask, self.position_rule)
         return types.SimpleNamespace(logits=logits, loss=None)
 
+    def score(self, frames: torch.Tensor, decoder_input_ids: torch.Tensor, decoder_attention_mask: Optional[torch.Tensor] = None
+              ) -> Dict[str, torch.Tensor]:
+        """Per-token entropy / surprisal / relative surprisal / suggested token of the teacher-forced pass `forward` runs
+        (see `ModelEngine.score_tokens`); encodes the frames per call, as `forward` does."""
+        B = frames.shape[0]
+        if decoder_input_ids.shape[0] != B:
+            raise ValueError(f"{decoder_input_ids.shape[0]} decoder rows for {B} windows of frames")
+        if B > self.engine.max_windows:
+            raise ValueError(f"{B} windows; this engine was built with max_windows={self.engine.max_windows}")
+        self.engine._score_args(list(range(B)), decoder_input_ids, decoder_attention_mask)   # reject before the encoder runs
+        self.engine.encode(frames.to(self.device, torch.float32), slot_begin=0)
+        return self.engine.score_tokens(list(range(B)), decoder_input_ids, decoder_attention_mask, self.position_rule)
+
     __call__ = forward

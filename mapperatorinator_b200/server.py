@@ -95,3 +95,20 @@ def model_forward(model, model_kwargs, generate_kwargs):
     out = model.forward(frames=model_kwargs["inputs"], decoder_input_ids=model_kwargs["decoder_input_ids"],
                         decoder_attention_mask=model_kwargs.get("decoder_attention_mask"))
     return out.logits.to(torch.float32).cpu()
+
+
+@torch.no_grad()
+def model_score(model, model_kwargs, generate_kwargs):
+    """MaiMod's scoring of given tokens (processor.py:511-525) on the teacher-forced pass `model_forward` runs, reduced on the
+    device: takes `model_forward`'s arguments and returns a dict of CPU tensors [B, L] indexed by the scored token (`entropy`,
+    `surprisal`, `relative`, `suggested`; see `ModelEngine.score_tokens`), so the caller slices `[start + padding, end + padding)`
+    where it sliced the logits at `[start + padding - 1, end + padding - 1)`.  `precision` is accepted and ignored (fp32).
+    A guided call (`cfg_scale > 1` with a negative prompt) is refused: the reference repeats the decoder rows but not the frames
+    there, which is not a pass worth mirroring."""
+    generate_kwargs = dict(generate_kwargs)
+    generate_kwargs.pop("precision", None)
+    if generate_kwargs.get("cfg_scale", 1.0) > 1.0 and model_kwargs.get("negative_prompt") is not None:
+        raise ValueError("model_score does not run a guided (cfg_scale > 1, negative prompt) teacher-forced pass")
+    out = model.score(frames=model_kwargs["inputs"], decoder_input_ids=model_kwargs["decoder_input_ids"],
+                      decoder_attention_mask=model_kwargs.get("decoder_attention_mask"))
+    return {k: v.cpu() for k, v in out.items()}
