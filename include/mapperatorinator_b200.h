@@ -264,6 +264,22 @@ int mb200_op_layernorm(const float* x, float* y, const float* w, const float* b,
 int mb200_op_attention(const float* q, const float* k, const float* v, float* o, int32_t B, int32_t H, int32_t Tq, int32_t Tk,
                        float scale, int32_t mask_mode, int32_t q_pos0, const uint8_t* key_valid, int32_t band,
                        const uint8_t* dense_mask, void* cuda_stream);
+/* One split-KV decode-attention phase of the token loop (decode.cu), through the engine's own launch functions and split plan.
+ * q [rows, H*64] already scaled; kv: K|V cache [slots, t_max, 2*H*64] (token stride 2*H*64, V at offset H*64); row_slot [rows] cache
+ * row of each decoder row (null = row r); out [rows, H*64] merged heads.  All pointers are DEVICE except ragged_cur_len /
+ * ragged_max_length (host).
+ *   self attention (fixed_len == 0): keys [0, cur_len); the split plan is that of max_length (one 128-key split up to 128, else
+ *     64-key splits); key_valid [rows, key_valid_ld] masks prompt positions t < prompt_len (null = all valid); kv_src [rows,
+ *     kv_src_ld] optional source-row table (beam search: key t of row r lives in cache row kv_src[r][t]);
+ *   cross attention (fixed_len > 0): keys [0, fixed_len) in 64-key splits;
+ *   ragged (ragged_cur_len and ragged_max_length given, host int32 [rows]): row r attends to its own cur_len keys with the plan of its
+ *     own max_length, no prompt mask, row_slot null;
+ *   form: 0 the engine's choice, 1 the CTA body with room for 128 keys, 2 the CTA body with 64, 3 the one-warp batch form.
+ * Synchronises the stream before it returns. */
+int mb200_op_decode_attention(const float* q, const float* kv, int32_t slots, int32_t t_max, int32_t H, int32_t rows, const int32_t* row_slot,
+                              int32_t cur_len, int32_t prompt_len, const uint8_t* key_valid, int64_t key_valid_ld, int32_t max_length,
+                              int32_t fixed_len, const int32_t* kv_src, int64_t kv_src_ld, const int32_t* ragged_cur_len,
+                              const int32_t* ragged_max_length, int32_t form, float* out, void* cuda_stream);
 /* Tuning / tests: tensor-core (wgmma, 3xTF32) flash attention on or off, and the minimum number of queries for which it is used
    (attention_tc.cu; replaces the SIMT kernel for the encoder self-attention of HF modeling_whisper.py:286-358 and the DiT band of
    osu_diffusion/utils/models.py:145-151). */

@@ -56,7 +56,7 @@ ABI_SYMBOLS = [
     "mb200_dit_sample_loop", "mb200_dit_set_option", "mb200_dit_set_sliders", "mb200_dit_apply_sliders",
     "mb200_launch_count", "mb200_model_set_option", "mb200_model_profile_step", "mb200_model_read_trace", "mb200_model_mega_stats", "mb200_model_logits_chain",
     "mb200_model_beam_step",
-    "mb200_op_gemm", "mb200_op_gemm_tc", "mb200_set_tensor_cores", "mb200_op_layernorm", "mb200_op_attention", "mb200_set_attention_tc", "mb200_audio_out_frames", "mb200_audio_ingest",
+    "mb200_op_gemm", "mb200_op_gemm_tc", "mb200_set_tensor_cores", "mb200_op_layernorm", "mb200_op_attention", "mb200_op_decode_attention", "mb200_set_attention_tc", "mb200_audio_out_frames", "mb200_audio_ingest",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -111,6 +111,7 @@ def load() -> C.CDLL:
     lib.mb200_op_layernorm.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, vp]
     lib.mb200_op_attention.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, f32, i32, i32, vp, i32, vp, vp]
     lib.mb200_set_attention_tc.argtypes = [i32, i32]
+    lib.mb200_op_decode_attention.argtypes = [vp, vp, i32, i32, i32, i32, vp, i32, i32, vp, i64, i32, i32, vp, i64, vp, vp, i32, vp, vp]
     lib.mb200_audio_out_frames.argtypes = [i64, i32, i32]
     lib.mb200_audio_out_frames.restype = i64
     lib.mb200_audio_ingest.argtypes = [vp, i64, i32, i32, i32, i32, vp, vp, vp]

@@ -1,5 +1,7 @@
 // C-ABI glue: error channel, the mel stage handle, and kernel-level entry points used by the parity tests.
+#include <algorithm>
 #include <string>
+#include <vector>
 
 #include "../../include/mapperatorinator_b200.h"
 #include "common.cuh"
@@ -109,6 +111,85 @@ extern "C" int mb200_op_attention(const float* q, const float* k, const float* v
     }
     return 0;
 }
+
+// One decode-attention phase through launch_decode_attention / launch_decode_attention_ragged, with the scratch a token step gives them
+// (call state, split partials, tickets) owned here.
+#define OP_TRY(expr) do { int _s = (expr); if (_s) return _s; } while (0)
+namespace {
+struct OpScratch {
+    void* p = nullptr; size_t bytes = 0;
+    int ensure(size_t need) {
+        if (need <= bytes) return 0;
+        if (p) cudaFree(p);
+        p = nullptr; bytes = 0;
+        MB_CUDA_CHECK(cudaMalloc(&p, need));
+        bytes = need;
+        return 0;
+    }
+};
+}  // namespace
+
+extern "C" int mb200_op_decode_attention(const float* q, const float* kv, int32_t slots, int32_t t_max, int32_t H, int32_t rows,
+                                         const int32_t* row_slot, int32_t cur_len, int32_t prompt_len, const uint8_t* key_valid,
+                                         int64_t key_valid_ld, int32_t max_length, int32_t fixed_len, const int32_t* kv_src, int64_t kv_src_ld,
+                                         const int32_t* ragged_cur_len, const int32_t* ragged_max_length, int32_t form, float* out,
+                                         void* stream) {
+    MB_REQUIRE(q && kv && out, "null argument");
+    MB_REQUIRE(rows >= 1 && H >= 1 && slots >= 1 && t_max >= 1, "rows, heads, slots and cache length must be positive");
+    const bool ragged = ragged_cur_len != nullptr;
+    MB_REQUIRE(ragged == (ragged_max_length != nullptr), "a ragged call gives both per-row cur_len and max_length");
+    MB_REQUIRE(!ragged || (fixed_len == 0 && !kv_src && form == ATTN_FORM_DEFAULT), "the ragged kernel is self attention without a table");
+    MB_REQUIRE(!kv_src || fixed_len == 0, "the source-row table applies to self attention");
+    const long long d = (long long)H * 64;
+    DecAttnParams a{};
+    a.q = q; a.q_ld = d; a.kc = kv; a.vc = kv + d; a.row_stride = (long long)t_max * 2 * d; a.tok_stride = 2 * d;
+    a.key_valid = key_valid; a.key_valid_ld = key_valid_ld;
+    a.kv_src = kv_src; a.kv_src_ld = kv_src_ld;
+    a.rows = rows; a.H = H; a.out = out; a.out_ld = d;
+    GenState gs{};
+    std::vector<RowState> rs;
+    if (ragged) {
+        gs.n_req = rows;
+        rs.resize(rows);
+        int S = 1;
+        for (int r = 0; r < rows; ++r) {
+            MB_REQUIRE(ragged_cur_len[r] >= 1 && ragged_cur_len[r] <= ragged_max_length[r] && ragged_max_length[r] <= t_max,
+                       "need 1 <= cur_len <= max_length <= cache length in every row");
+            rs[r].cur_len = ragged_cur_len[r]; rs[r].prompt_len = 0; rs[r].max_length = ragged_max_length[r];
+            S = std::max(S, self_splits(ragged_max_length[r]));
+        }
+        MB_REQUIRE(!row_slot, "a ragged row reads its own cache row");
+        a.n_splits = S;                                  // the grid: the largest plan of the call
+        a.chunk = self_split_chunk(S);                   // (not read by the ragged kernel)
+    } else if (fixed_len > 0) {
+        MB_REQUIRE(fixed_len <= t_max, "fixed_len exceeds the cache length");
+        a.fixed_len = fixed_len; a.chunk = 64; a.n_splits = (fixed_len + 63) / 64;      // cross attention: 64-key splits
+        gs.prompt_len = prompt_len;
+    } else {
+        MB_REQUIRE(cur_len >= 1 && cur_len <= max_length && max_length <= t_max, "need 1 <= cur_len <= max_length <= cache length");
+        MB_REQUIRE(prompt_len >= 0 && prompt_len <= cur_len, "need 0 <= prompt_len <= cur_len");
+        a.n_splits = self_splits(max_length);
+        a.chunk = self_split_chunk(a.n_splits);
+        gs.cur_len = cur_len; gs.prompt_len = prompt_len; gs.max_length = max_length;
+    }
+    a.row_slot = row_slot;
+    cudaStream_t st = (cudaStream_t)stream;
+    static OpScratch op_state, op_parts, op_tickets;
+    const size_t n_units = (size_t)rows * H * a.n_splits;
+    OP_TRY(op_state.ensure(sizeof(GenState) + (size_t)rows * sizeof(RowState)));
+    OP_TRY(op_parts.ensure(n_units * 66 * sizeof(float)));
+    OP_TRY(op_tickets.ensure((size_t)rows * H * sizeof(int)));
+    MB_CUDA_CHECK(cudaMemcpyAsync(op_state.p, &gs, sizeof(GenState), cudaMemcpyHostToDevice, st));
+    if (ragged) MB_CUDA_CHECK(cudaMemcpyAsync(reinterpret_cast<GenState*>(op_state.p) + 1, rs.data(), rs.size() * sizeof(RowState), cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(op_tickets.p, 0, (size_t)rows * H * sizeof(int), st));
+    a.st = reinterpret_cast<const GenState*>(op_state.p);
+    a.part_o = reinterpret_cast<float*>(op_parts.p); a.part_ml = a.part_o + n_units * 64;
+    a.ticket = reinterpret_cast<int*>(op_tickets.p);
+    OP_TRY(ragged ? launch_decode_attention_ragged(a, st, false) : launch_decode_attention(a, st, false, form));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));      // the host-side state above goes out of scope
+    return 0;
+}
+
 // tuning / tests: minimum query count for the tensor-core attention path (0 disables it)
 extern "C" int mb200_set_attention_tc(int32_t enabled, int32_t min_queries) {
     g_attn_tc_enabled = enabled; g_attn_tc_min_t = min_queries;

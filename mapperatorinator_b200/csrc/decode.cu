@@ -86,7 +86,7 @@ __global__ void __launch_bounds__(128, 4) decode_attention_ragged_kernel(DecAttn
     const long long shift = ((long long)r * p.H + h) * (p.n_splits - S);
     p.part_o += shift * 64; p.part_ml += shift * 2;
     p.n_splits = S;
-    p.chunk = S == 1 ? 128 : 64;
+    p.chunk = self_split_chunk(S);
     AttnRegs<4, KMAX> regs;
     decode_attention_load<4, KMAX, false>(p, s, h, r, r, L, 0, threadIdx.x, regs);
     decode_attention_body<4, KMAX, false>(p, s, h, r, r, L, 0, sc, red, stat, threadIdx.x, regs);
@@ -204,11 +204,23 @@ int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged)
     }
 }
 
-int launch_decode_attention(const DecAttnParams& p, cudaStream_t stream, bool pdl) {
+int launch_decode_attention(const DecAttnParams& p, cudaStream_t stream, bool pdl, int form) {
     MB_REQUIRE(p.chunk > 0 && p.chunk <= 128, "decode attention chunk must be in (0, 128]");
     MB_REQUIRE(p.out && p.ticket, "decode attention needs the merged-output buffer and its tickets");
+    MB_REQUIRE(form >= ATTN_FORM_DEFAULT && form <= ATTN_FORM_WARP, "unknown decode attention form");
+    MB_REQUIRE(form != ATTN_FORM_CTA64 || p.chunk <= 64, "the KMAX 64 body cannot hold a chunk of more than 64 keys");
+    MB_REQUIRE(form != ATTN_FORM_WARP || !p.kv_src, "the one-warp body has no source-row table");
     if (p.rows <= 0) return 0;
     g_prof_class = 1;
+    const dim3 grid(p.n_splits, p.H, p.rows);
+    if (form == ATTN_FORM_CTA128)
+        return p.kv_src ? launch_with_attrs(decode_attention_kernel<128, true>, grid, dim3(128), 0, stream, pdl, p)
+                        : launch_with_attrs(decode_attention_kernel<128>, grid, dim3(128), 0, stream, pdl, p);
+    if (form == ATTN_FORM_CTA64)
+        return p.kv_src ? launch_with_attrs(decode_attention_kernel<64, true>, grid, dim3(128), 0, stream, pdl, p)
+                        : launch_with_attrs(decode_attention_kernel<64>, grid, dim3(128), 0, stream, pdl, p);
+    if (form == ATTN_FORM_WARP)
+        return launch_with_attrs(decode_attention_warp_kernel, dim3((p.rows * p.H * p.n_splits + 7) / 8), dim3(256), 0, stream, pdl, p);
     // Default: one CTA per unit with everything prefetched (the megakernel's phase body).  MB200_ATTN_BATCH=1 selects the
     // one-warp-per-unit form for rows > 2 — the same arithmetic value for value (parity-tested), kept as the starting point for a
     // persistent multi-unit kernel.

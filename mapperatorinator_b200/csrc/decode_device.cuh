@@ -33,10 +33,19 @@ constexpr long long LL_SPIN_LIMIT = 1ll << 24;      // ~ seconds; a dataflow wai
 // exchange buffer is taken), bit 2 = GEMV phases skip their multiply-reduce.  Any bit set -> the tokens are garbage, the TIMING tells
 // which part of a phase the time goes to.
 static __constant__ int c_ll_debug = 0;
-__device__ __forceinline__ bool ll_spin_check(long long& spin, int* err) {
+// The wait that times out first also records where it was: err[1] = CTA, err[2] = thread, err[3] = the tag it expected, i.e. the step
+// (tag / 128 - 1) and the phase (tag % 128 - 1) whose output never arrived.  Waits that give up because the flag is already raised
+// record nothing.
+__device__ __forceinline__ bool ll_spin_check(long long& spin, int* err, unsigned tag) {
     if (c_ll_debug & 2) return false;
     if (c_ll_sleep_ns > 0) __nanosleep((unsigned)c_ll_sleep_ns);
-    if ((++spin & 0x3FF) == 0 && (spin > LL_SPIN_LIMIT || *reinterpret_cast<volatile int*>(err) != 0)) { atomicCAS(err, 0, 4); return false; }
+    if ((++spin & 0x3FF) == 0 && (spin > LL_SPIN_LIMIT || *reinterpret_cast<volatile int*>(err) != 0)) {
+        if (spin > LL_SPIN_LIMIT && atomicCAS(err, 0, 4) == 0) {
+            err[1] = (int)blockIdx.x; err[2] = (int)threadIdx.x; err[3] = (int)tag;
+            __threadfence();
+        }
+        return false;
+    }
     return true;
 }
 __device__ __forceinline__ float ll_wait1(const ll_t* p, unsigned tag, int* err) {
@@ -45,7 +54,7 @@ __device__ __forceinline__ float ll_wait1(const ll_t* p, unsigned tag, int* err)
     while (true) {
         asm volatile("ld.relaxed.gpu.global.b64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
         if ((unsigned)(v >> 32) == tag) return __uint_as_float((unsigned)v);
-        if (!ll_spin_check(spin, err)) return 0.f;
+        if (!ll_spin_check(spin, err, tag)) return 0.f;
     }
 }
 __device__ __forceinline__ float2 ll_wait2(const ll_t* p, unsigned tag, int* err) {
@@ -54,7 +63,7 @@ __device__ __forceinline__ float2 ll_wait2(const ll_t* p, unsigned tag, int* err
     while (true) {
         ll_load2(p, a, b);
         if ((unsigned)(a >> 32) == tag && (unsigned)(b >> 32) == tag) return make_float2(__uint_as_float((unsigned)a), __uint_as_float((unsigned)b));
-        if (!ll_spin_check(spin, err)) return make_float2(0.f, 0.f);
+        if (!ll_spin_check(spin, err, tag)) return make_float2(0.f, 0.f);
     }
 }
 __device__ __forceinline__ float4 ll_wait4(const ll_t* p, unsigned tag, int* err) {        // p 32-byte aligned
@@ -65,7 +74,7 @@ __device__ __forceinline__ float4 ll_wait4(const ll_t* p, unsigned tag, int* err
         ll_load2(p + 2, c, d);
         if ((unsigned)(a >> 32) == tag && (unsigned)(b >> 32) == tag && (unsigned)(c >> 32) == tag && (unsigned)(d >> 32) == tag)
             return make_float4(__uint_as_float((unsigned)a), __uint_as_float((unsigned)b), __uint_as_float((unsigned)c), __uint_as_float((unsigned)d));
-        if (!ll_spin_check(spin, err)) return make_float4(0.f, 0.f, 0.f, 0.f);
+        if (!ll_spin_check(spin, err, tag)) return make_float4(0.f, 0.f, 0.f, 0.f);
     }
 }
 
@@ -718,7 +727,7 @@ static __device__ __forceinline__ void sample_poll_ll(const SampleParams& p, int
                         const int v = tid + (j0 + j) * NT;
                         if (v < V) ok = ok && (unsigned)(w[j] >> 32) == in_tag;
                     }
-                    if (ok || !ll_spin_check(spin, p.ll_err)) break;
+                    if (ok || !ll_spin_check(spin, p.ll_err, in_tag)) break;
                     __nanosleep(96);      // one CTA spinning on 29 KB of lines that 147 CTAs are storing into: back off so the stores get through
                 }
                 // (flags first, all at once: a load behind a conditional cannot be moved above the previous element's store by the compiler,

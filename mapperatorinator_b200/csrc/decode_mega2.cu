@@ -159,9 +159,9 @@ __device__ __forceinline__ void m2_attention_unit(const DecAttnParams& p, const 
     ll_t* att = ll.att + (long long)r * d + h * 64;
     if (nk <= 0) {                                                 // empty split (uniform across the CTA)
         if (p.n_splits == 1) { if (tid < 64) for (int rep = 0; rep < ll.reps; ++rep) ll_store(att + rep * ll.x_rep + tid, 0.f, out_tag); return; }
-        if (tid < 64) ll_store(part + tid, 0.f, out_tag);
-        if (tid == 0) { ll_store(part + 64, -INFINITY, out_tag); ll_store(part + 65, 0.f, out_tag); }
-        stat[0] = -INFINITY; stat[1] = 0.f;
+        // No partial: the merge knows the split is empty (m_s = -inf, l_s = 0 contributes nothing) and does not poll it.  A store here
+        // would depend on no input of this token, so a CTA with nothing else to wait for (no GEMV rows, no other unit) could run ahead
+        // into the next layer's self attention and overwrite this slot before this phase's merge had read it.
         return;
     }
     const int tok = (int)p.tok_stride;
@@ -181,7 +181,7 @@ __device__ __forceinline__ void m2_attention_unit(const DecAttnParams& p, const 
         while (true) {
             ll_load2(kn + lane * 2, w[0], w[1]);
             ll_load2(kn + d + lane * 2, w[2], w[3]);
-            if (ll_tag_ok4(w[0], w[1], w[2], w[3], in_tag) || !ll_spin_check(spin, err)) break;
+            if (ll_tag_ok4(w[0], w[1], w[2], w[3], in_tag) || !ll_spin_check(spin, err, in_tag)) break;
         }
         kns[lane * 2] = ll_val(w[0]); kns[lane * 2 + 1] = ll_val(w[1]);
         vns[lane * 2] = ll_val(w[2]); vns[lane * 2 + 1] = ll_val(w[3]);
@@ -276,17 +276,20 @@ __device__ __forceinline__ void m2_attention_unit(const DecAttnParams& p, const 
 }
 
 // merge of the S split partials of (row r, head h) by the CTA that computed split 0: splits visited in index order,
-// out = sum_s w_s o_s / sum_s w_s l_s with w_s = exp(m_s - max m) — decode_attention_merge's arithmetic, operands polled
-__device__ __forceinline__ void m2_attention_merge(const DecAttnParams& p, const MegaLL& ll, int h, int r, unsigned tag, float* msh /* >= 2 * 32 floats of shared memory */,
-                                                   int tid, int* err) {
+// out = sum_s w_s o_s / sum_s w_s l_s with w_s = exp(m_s - max m) — decode_attention_merge's arithmetic, operands polled.
+// Splits at or beyond key L are empty: they publish no partial and enter the sums as (m, l) = (-inf, 0), which is what the per-phase
+// merge reads for them (same bits).
+__device__ __forceinline__ void m2_attention_merge(const DecAttnParams& p, const MegaLL& ll, int h, int r, int L, unsigned tag,
+                                                   float* msh /* >= 2 * 32 floats of shared memory */, int tid, int* err) {
     // called by the WHOLE CTA (uniform).  Threads 64 .. 64+S-1 poll the (m, l) pair of one split each into shared memory, threads 0..63
-    // poll their output dim of every split (S <= 8: one batch; beyond that: rolled), then 64 threads combine.
+    // poll their output dim of every split (S <= 16: one batch; beyond that: rolled), then 64 threads combine.
     const int S = p.n_splits, d = p.H * 64;
+    const int S_live = min(S, (L + p.chunk - 1) / p.chunk);        // splits that hold keys
     const ll_t* base = ll.part + ((long long)r * p.H + h) * ll.max_splits * M2_PART;
     for (int s0 = 0; s0 < S; s0 += 32) {
         const int s = s0 + (tid - 64);
         if (tid >= 64 && tid < 96 && s < S) {
-            const float2 mv = ll_wait2(base + (long long)s * M2_PART + 64, tag, err);
+            const float2 mv = s < S_live ? ll_wait2(base + (long long)s * M2_PART + 64, tag, err) : make_float2(-INFINITY, 0.f);
             if (s < 32) { msh[s] = mv.x; msh[32 + s] = mv.y; }
         }
     }
@@ -299,14 +302,14 @@ __device__ __forceinline__ void m2_attention_merge(const DecAttnParams& p, const
             bool ok = true;
 #pragma unroll
             for (int s = 0; s < SB; ++s)
-                if (s < S) asm volatile("ld.relaxed.gpu.global.b64 %0, [%1];" : "=l"(oo[s]) : "l"(base + (long long)s * M2_PART + tid) : "memory");
+                if (s < S_live) asm volatile("ld.relaxed.gpu.global.b64 %0, [%1];" : "=l"(oo[s]) : "l"(base + (long long)s * M2_PART + tid) : "memory");
 #pragma unroll
             for (int s = 0; s < SB; ++s)
-                if (s < S) ok = ok && (unsigned)(oo[s] >> 32) == tag;
-            if (ok || !ll_spin_check(spin, err)) break;
+                if (s < S_live) ok = ok && (unsigned)(oo[s] >> 32) == tag;
+            if (ok || !ll_spin_check(spin, err, tag)) break;
         }
 #pragma unroll
-        for (int s = 0; s < SB; ++s) ov[s] = s < S ? ll_val(oo[s]) : 0.f;
+        for (int s = 0; s < SB; ++s) ov[s] = s < S_live ? ll_val(oo[s]) : 0.f;
     }
     __syncthreads();
     if (tid >= 64) return;
@@ -327,7 +330,7 @@ __device__ __forceinline__ void m2_attention_merge(const DecAttnParams& p, const
 #pragma unroll 1
         for (int s = 0; s < S; ++s) mmax = fmaxf(mmax, msh[s]);
 #pragma unroll 1
-        for (int s = 0; s < S; ++s) {
+        for (int s = 0; s < S_live; ++s) {                   // (empty splits: l = 0, nothing to add)
             const float o1 = ll_wait1(base + (long long)s * M2_PART + tid, tag, err);
             if (msh[32 + s] > 0.f) {
                 const float w = expf(msh[s] - mmax);
@@ -543,7 +546,7 @@ __device__ __forceinline__ void m3_rw_tail(const Mega2Params& mp, const Mega2Pha
 #pragma unroll
             for (int b = 0; b < NB; ++b)
                 if (on[b][0]) ok = ok && ll_tag_ok4(w[b][0][0], w[b][0][1], w[b][0][2], w[b][0][3], in_tag);
-            if (ok || !ll_spin_check(spin, err)) break;
+            if (ok || !ll_spin_check(spin, err, in_tag)) break;
 #pragma unroll
             for (int b = 0; b < NB; ++b)
                 if (on[b][0]) {
@@ -786,7 +789,7 @@ __device__ __forceinline__ void m3_gemv_phase(const Mega2Params& mp, const Mega2
 #pragma unroll
                 for (int s = 0; s < M3_NS; ++s)
                     if (on[b][s]) ok = ok && ll_tag_ok4(w[b][s][0], w[b][s][1], w[b][s][2], w[b][s][3], in_tag);
-            if (ok || !ll_spin_check(spin, err)) break;
+            if (ok || !ll_spin_check(spin, err, in_tag)) break;
 #pragma unroll
             for (int b = 0; b < NB; ++b)
 #pragma unroll
@@ -1021,7 +1024,7 @@ __global__ void __launch_bounds__(M2_THREADS, 1) decode_megakernel_ll(Mega2Param
                     m2_attention_unit(a, mp.ll, is_self, s, h, r, slot, L, P, in_tag, out_tag, sm.u.attn.sc, sm.u.attn.red, sm.u.attn.stat, sm.u.attn.qs,
                                       sm.u.attn.kns, sm.u.attn.vns, tid, areg, err, tr);
                     if (tr && tid == 0) tr[5] = (unsigned long long)clock64();
-                    if (a.n_splits > 1 && s == 0) { __syncthreads(); m2_attention_merge(a, mp.ll, h, r, out_tag, sm.u.attn.sc, tid, err); if (tr && tid == 0) tr[6] = (unsigned long long)clock64(); }
+                    if (a.n_splits > 1 && s == 0) { __syncthreads(); m2_attention_merge(a, mp.ll, h, r, L, out_tag, sm.u.attn.sc, tid, err); if (tr && tid == 0) tr[6] = (unsigned long long)clock64(); }
                     __syncthreads();
                 }
             } else {

@@ -668,7 +668,7 @@ static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaSt
             a.q = q; a.q_ld = d; a.kc = skv; a.vc = skv + d; a.row_stride = self_row; a.tok_stride = 2 * d; a.row_slot = nullptr;
             a.fixed_len = 0; a.st = gs; a.key_valid = m->g_keyvalid.as<unsigned char>(); a.key_valid_ld = c.tgt_seq_len;
             a.part_o = po; a.part_ml = pml; a.rows = rows; a.H = H; a.n_splits = n_splits_self;
-            a.chunk = n_splits_self == 1 ? 128 : chunk;      // contexts up to 128 tokens: one split per head, no merge step
+            a.chunk = self_split_chunk(n_splits_self);      // contexts up to 128 tokens: one split per head, no merge step
             a.out = attn; a.out_ld = d; a.ticket = ticket;
             if (beam) { a.kv_src = beam->kv_src; a.kv_src_ld = beam->kv_src_ld; }
             if (ragged) {
@@ -842,6 +842,7 @@ static int run_megakernel2(mb200_model* m, int rows, int B, int n_splits_self, i
     MB_TRY(launch_megakernel2(mp, m->num_sms, st));
     MB_CUDA_CHECK(cudaEventRecord(m->mega_ev[1], st));
     MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 1, m->g_megasync.as<int>() + 8, 4, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 4, m->g_megasync.as<int>() + 9, 12, cudaMemcpyDeviceToHost, st));   // where a timed-out wait was
     MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 3, &m->g_state.as<GenState>()->cur_len, 4, cudaMemcpyDeviceToHost, st));
     MB_TRY(before_sync());
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -849,6 +850,13 @@ static int run_megakernel2(mb200_model* m, int rows, int B, int n_splits_self, i
         float ms = 0.f;
         MB_CUDA_CHECK(cudaEventElapsedTime(&ms, m->mega_ev[0], m->mega_ev[1]));
         m->mega_ms += ms; m->mega_launches += 1; m->mega_tokens += m->h_flag[3] - m->h_flag[2];
+    }
+    if (m->h_flag[1] == 4) {
+        const unsigned tag = (unsigned)m->h_flag[6];
+        MB_REQUIRE(false, "dataflow megakernel: a wait for tagged data timed out (CTA " + std::to_string(m->h_flag[4]) + ", thread " +
+                              std::to_string(m->h_flag[5]) + ", expected tag " + std::to_string(tag) + " = step " + std::to_string((int)(tag / 128) - 1) +
+                              " phase " + std::to_string((int)(tag % 128) - 1) + " of " + std::to_string(mp.n_phases) + ", splits " +
+                              std::to_string(n_splits_self) + ", rows " + std::to_string(rows) + ")");
     }
     MB_REQUIRE(m->h_flag[1] == 0, m->h_flag[1] == 2 ? "dataflow megakernel: weight copy timed out" : "dataflow megakernel: a wait for tagged data timed out");
     return 0;

@@ -187,6 +187,8 @@ __host__ __device__ inline RowState* ragged_rows(GenState* st) { return reinterp
 // split-KV layout of the self-attention cache of ONE call: one 128-key split while the context fits, 64-key splits beyond.  A ragged
 // row keeps the plan of its own max_length, whatever its neighbours need: its partials and their merge order are its own call's.
 __host__ __device__ inline int self_splits(int max_length) { return max_length <= 128 ? 1 : (max_length + 63) / 64; }
+// keys per split of that plan: the single split holds all 128, every plan of several splits cuts 64-key chunks
+__host__ __device__ inline int self_split_chunk(int n_splits) { return n_splits == 1 ? 128 : 64; }
 
 struct SampleConfig {        // device-resident, rewritten by the host once per generate() call
     int B;                   // un-doubled batch rows
@@ -247,7 +249,10 @@ struct DecAttnParams {
     int* ticket;                                    // [rows, H] arrival counters, zero on entry, reset by the last arriver
     const int* kv_src; long long kv_src_ld;         // beam search: [rows, kv_src_ld] cache row holding key position t of row r (null = row r)
 };
-int launch_decode_attention(const DecAttnParams& p, cudaStream_t stream, bool pdl);
+// Which kernel body runs the units.  DEFAULT is the engine's own choice (the CTA body, KMAX from the chunk; the one-warp batch form for
+// rows > 2 when MB200_ATTN_BATCH is set); the others force one body — the kernel-level tests compare them bit for bit.
+enum DecAttnForm : int { ATTN_FORM_DEFAULT = 0, ATTN_FORM_CTA128 = 1, ATTN_FORM_CTA64 = 2, ATTN_FORM_WARP = 3 };
+int launch_decode_attention(const DecAttnParams& p, cudaStream_t stream, bool pdl, int form = ATTN_FORM_DEFAULT);
 // Ragged self attention: p.st heads a ragged state; row r attends to its own cur_len keys with the split plan of its own max_length.
 // p.n_splits = splits of the grid (the largest plan of the call; also the row stride of the partials); p.chunk is not read.
 int launch_decode_attention_ragged(const DecAttnParams& p, cudaStream_t stream, bool pdl);

@@ -67,3 +67,34 @@ def attention(q, k, v, heads, scale=1.0, mask="none", q_pos0=0, key_valid=None, 
     _lib.check(lib.mb200_op_attention(_ptr(q), _ptr(k), _ptr(v), _ptr(o), B, heads, Tq, Tk, float(scale), MASK[mask], int(q_pos0),
                                       _ptr(key_valid), int(band), _ptr(dense_mask), _stream()))
     return o
+
+
+DECODE_ATTENTION_FORMS = {"default": 0, "cta128": 1, "cta64": 2, "warp": 3}
+
+
+def decode_attention(q, kv, heads, *, row_slot=None, cur_len=0, prompt_len=0, key_valid=None, max_length=0, fixed_len=0, kv_src=None,
+                     ragged_cur_len=None, ragged_max_length=None, form="default"):
+    """One split-KV decode-attention phase of the token loop (`mb200_op_decode_attention`).
+
+    q (rows, H*64) already scaled; kv the engine's K|V cache (slots, T_max, 2*H*64); row_slot int32 (rows,) cache row per decoder row;
+    key_valid uint8 (rows, ld) prompt mask; kv_src int32 (rows, ld) source-row table.  Self attention over keys [0, cur_len) with the
+    split plan of `max_length`, cross attention over [0, fixed_len) when fixed_len > 0, or a ragged launch when the per-row lists
+    `ragged_cur_len` / `ragged_max_length` are given.  Returns the merged heads (rows, H*64)."""
+    import ctypes as C
+    lib = _lib.load()
+    q, kv = _f32c(q), _f32c(kv)
+    rows = q.shape[0]
+    slots, t_max, _ = kv.shape
+    for t, dt in ((row_slot, torch.int32), (key_valid, torch.uint8), (kv_src, torch.int32)):
+        assert t is None or (t.is_cuda and t.dtype == dt and t.is_contiguous())
+    out = torch.empty_like(q)
+    rc = rm = None
+    if ragged_cur_len is not None:
+        rc = (C.c_int32 * rows)(*[int(x) for x in ragged_cur_len])
+        rm = (C.c_int32 * rows)(*[int(x) for x in ragged_max_length])
+    _lib.check(lib.mb200_op_decode_attention(_ptr(q), _ptr(kv), slots, t_max, int(heads), rows, _ptr(row_slot), int(cur_len), int(prompt_len),
+                                             _ptr(key_valid), key_valid.shape[1] if key_valid is not None else 0, int(max_length),
+                                             int(fixed_len), _ptr(kv_src), kv_src.shape[1] if kv_src is not None else 0,
+                                             None if rc is None else C.cast(rc, C.c_void_p), None if rm is None else C.cast(rm, C.c_void_p),
+                                             DECODE_ATTENTION_FORMS[form], _ptr(out), _stream()))
+    return out

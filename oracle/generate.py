@@ -199,7 +199,8 @@ def teacher_forced_check(w, cfg, layout, pcm: torch.Tensor, full_ids: torch.Tens
     `full_ids` (B = 1, prompt + generated), then the processor chain replayed position by position on those logits
     (server.py:106-134 order, same `Processors` as `model_generate`).  For every generated position t it asks whether
     argmax(processed scores) == full_ids[t] and records the smallest top-1 / top-2 gap seen, so a disagreement can be told apart
-    from a near-tie.  Returns {"match", "n_checked", "first_divergence": None | {"index", "got", "want", "gap"}, "min_gap"}.
+    from a near-tie.  Returns {"match", "n_checked", "first_divergence": None | {"index", "got", "want", "gap"}, "min_gap",
+    "gaps", "mismatch"}: the top-1 / top-2 gap of every generated position and whether its token differs from the argmax.
     Greedy only (do_sample False), cfg_scale 1."""
     gk = dict(generate_kwargs)
     assert not gk.get("do_sample", False) and float(gk.get("cfg_scale", 1.0)) <= 1.0
@@ -213,14 +214,17 @@ def teacher_forced_check(w, cfg, layout, pcm: torch.Tensor, full_ids: torch.Tens
     mask[:, :prompt_len] = ids[:, :prompt_len].ne(layout.pad_id)
     logits = W.decoder_forward(st, ids[:, :L - 1], mask, position_rule)             # (1, L-1, V): row t-1 predicts token t
     pr = Processors(layout, 1, prompt_len, gk)
-    first, min_gap = None, float("inf")
+    first, min_gap, gaps, mismatch = None, float("inf"), [], []
     for t in range(prompt_len, L):
         scores = pr(ids[:, :t], logits[:, t - 1])
         top = torch.topk(scores[0], 2)
         gap = float(top.values[0] - top.values[1])
         min_gap = min(min_gap, gap)
+        gaps.append(gap)
         want = int(top.indices[0])
+        mismatch.append(want != int(ids[0, t]))
         if want != int(ids[0, t]) and first is None:
             got_score = float(scores[0, int(ids[0, t])])
             first = {"index": t, "got": int(ids[0, t]), "want": want, "gap": float(top.values[0]) - got_score}
-    return {"match": first is None, "n_checked": L - prompt_len, "first_divergence": first, "min_gap": min_gap}
+    return {"match": first is None, "n_checked": L - prompt_len, "first_divergence": first, "min_gap": min_gap, "gaps": gaps,
+            "mismatch": mismatch}

@@ -134,3 +134,91 @@ def test_greedy_ids_vs_oracle_teacher_forced_full_dims(full, layout):
             full_ids = torch.tensor([prompt + streams[i]])
             rep = go.teacher_forced_check(sd, cfg, layout, windows[i:i + 1], full_ids, len(prompt), gk_fn(i, len(prompt)))
             assert rep["match"], f"window {i}: {rep}"
+
+
+# ---- the token loop at the model's own max_length (2 048): every self-attention split plan, every driver -------------------------
+# max_length -> S = max_length <= 128 ? 1 : ceil(max_length / 64).  S = 11 is 132 attention units per row (one per SM of an H100), 12 is
+# the first plan with more units than CTAs, 17 the first past the dataflow merge's 16 in-flight splits, 32 the plan of every drop-in call.
+PLAN_LENGTHS = [128, 192, 640, 704, 705, 1024, 1025, 1408, 2048]
+DRIVERS = {"dataflow": 2, "megakernel": 1, "graph": 0}
+TOP2_GAP = 1e-4
+
+
+def _plan_case(max_length, rows):
+    """P = max_length - 17 random ids (built like cases.long_context_cases), min_new_tokens fixes the length: 16 tokens decode inside
+    the token loop at nearly full context.  rows == 2: the CFG pair (negative prompt of the same length)."""
+    from oracle import cases
+    P = max_length - 17
+    g = torch.Generator().manual_seed(max_length)
+    prompt = torch.randint(17, 3600, (1, P), generator=g)
+    prompt[0, :4] = torch.tensor([3700, 3705, 1, 9])
+    neg = None
+    if rows == 2:
+        neg = torch.randint(17, 3600, (1, P), generator=g)
+        neg[0, :4] = torch.tensor([3700, 3705, 1, 9])
+    gk = dict(cases.GK, max_length=max_length, min_new_tokens=max_length - P, lookback_time=0.0, lookahead_time=0.0, context_type="map",
+              cfg_scale=1.5 if rows == 2 else 1.0)
+    return prompt, neg, gk
+
+
+def _generate(model, layout, slot, prompt, neg, gk, driver):
+    model.engine.set_option("mega", DRIVERS[driver])
+    try:
+        return model.engine.generate([slot], prompt, None, layout, dict(gk), negative_prompt=neg)
+    finally:
+        model.engine.set_option("mega", 2)
+
+
+def _oracle_check(sd, cfg, layout, pcm, ids, P, gk, what):
+    """Teacher-forced CPU oracle on the GPU ids: every position whose top-2 gap exceeds TOP2_GAP must be the oracle's argmax.
+    Returns (positions under the gap, smallest gap) for the report."""
+    from oracle import generate as go
+    torch.set_num_threads(min(os.cpu_count() or 1, 16))
+    with torch.no_grad():
+        rep = go.teacher_forced_check(sd, cfg, layout, pcm, ids, P, gk)
+    gaps = np.asarray(rep["gaps"])
+    bad = [P + i for i, (g, m) in enumerate(zip(rep["gaps"], rep["mismatch"])) if m and g > TOP2_GAP]
+    near = int((gaps <= TOP2_GAP).sum())
+    print(f"{what}: {rep['n_checked']} positions checked, {near} with a top-2 gap <= {TOP2_GAP}, smallest gap {rep['min_gap']:.3e}")
+    assert not bad, f"{what}: mismatches at positions {bad[:10]} with top-2 gap > {TOP2_GAP} ({rep['first_divergence']})"
+    return near, rep["min_gap"]
+
+
+@pytest.mark.parametrize("max_length", PLAN_LENGTHS, ids=[f"ml{m}" for m in PLAN_LENGTHS])
+def test_split_plans_all_drivers_full_dims(full, layout, max_length):
+    """Every driver decodes every plan, and their ids are equal bit for bit: B = 1, and for S in {11, 22, 32} also the CFG pair
+    (264, 528, 768 attention units).  S in {11, 17, 32}: the dataflow ids also pass the teacher-forced oracle."""
+    from oracle import cases
+    cfg, sd, model = full
+    S = 1 if max_length <= 128 else (max_length + 63) // 64
+    pcm = cases.model_pcm(cfg, 1, 40 + max_length)
+    model.engine.encode(pcm.cuda(), slot_begin=0)
+    for rows in ((1, 2) if S in (11, 22, 32) else (1,)):
+        prompt, neg, gk = _plan_case(max_length, rows)
+        got = {drv: _generate(model, layout, 0, prompt, neg, gk, drv) for drv in DRIVERS}
+        for drv, ids in got.items():
+            assert ids.shape == (1, max_length), f"S {S} rows {rows} {drv}: shape {tuple(ids.shape)}"
+            assert torch.equal(ids[:, :prompt.shape[1]], prompt)
+            assert torch.equal(ids, got["graph"]), f"S {S} rows {rows}: {drv} differs from graph at {(ids != got['graph']).nonzero()[:4].tolist()}"
+        if rows == 1 and S in (11, 17, 32):
+            _oracle_check(sd, cfg, layout, pcm, got["dataflow"].cpu(), prompt.shape[1], gk, f"max_length {max_length} (S {S})")
+
+
+@pytest.mark.parametrize("P", [18, 50])
+def test_reference_call_shape_max_length_2048_full_dims(full, layout, P):
+    """The reference's own call: a bench-like prompt and max_length = tgt_seq_len = 2048, ~2 000 tokens through 32 splits.  Dataflow ids
+    equal graph ids; the P = 18 run also passes the teacher-forced oracle."""
+    from oracle import cases
+    cfg, sd, model = full
+    pcm = cases.model_pcm(cfg, 1, 70 + P)
+    model.engine.encode(pcm.cuda(), slot_begin=0)
+    cond = [3667, 3680, 3700, 3710, 3730, 3798, 3810, 3870, 3965, 3975, 3992, 4006, 4100, 3862, 3863, 3864, 1, 9]
+    g = torch.Generator().manual_seed(P)
+    prompt = torch.tensor([(cond + torch.randint(17, 3600, (P - len(cond),), generator=g).tolist())[:P]])
+    gk = dict(cases.GK, max_length=2048, min_new_tokens=2048 - P, lookback_time=0.0, lookahead_time=0.0, context_type="map")
+    a = _generate(model, layout, 0, prompt, None, gk, "dataflow")
+    b = _generate(model, layout, 0, prompt, None, gk, "graph")
+    assert a.shape == b.shape == (1, 2048)
+    assert torch.equal(a, b), f"dataflow differs from graph at {(a != b).nonzero()[:4].tolist()}"
+    if P == 18:
+        _oracle_check(sd, cfg, layout, pcm, a.cpu(), P, gk, f"P {P}, max_length 2048")

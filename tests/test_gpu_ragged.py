@@ -190,8 +190,10 @@ def test_decode_songs_ragged_equals_decode_windows_per_song(tiny16, layout):
 
 
 def _full_requests(n, new=64):
+    """n requests with prompt lengths spread over 17..600 (the last one: max_length 664, 11 self-attention splits), then two at the
+    model's long plans: max_length 1025 (17 splits) and 2048 (32 splits, the reference's own max_length)."""
     g = torch.Generator().manual_seed(n)
-    lens = torch.linspace(17, 600, n).round().long().tolist()
+    lens = torch.linspace(17, 600, n).round().long().tolist() + [1025 - new, 2048 - new]
     reqs = []
     for r, P in enumerate(lens):
         prompt = torch.randint(17, 3600, (1, P), generator=g)
@@ -203,21 +205,20 @@ def _full_requests(n, new=64):
 
 
 def test_ragged_equals_batch1_calls_full_dims(layout):
-    """whisper-small dimensions: 8 and 16 requests with prompt lengths spread over 17..600 on resident encoder slots, 64 tokens each,
-    equal their batch-1 calls."""
+    """whisper-small dimensions: 9 and 18 requests with prompt lengths spread over 17..600 plus max_length 1025 and 2048 on resident
+    encoder slots, 64 tokens each, equal their batch-1 calls on the default driver."""
     from mapperatorinator_b200 import v29_model_config
     from mapperatorinator_b200.modeling import B200Mapperatorinator
     from mapperatorinator_b200.weights import init_model_state_dict
     cfg = v29_model_config()
-    model = B200Mapperatorinator(cfg, init_model_state_dict(cfg, 0), max_windows=16, max_batch=16)
+    model = B200Mapperatorinator(cfg, init_model_state_dict(cfg, 0), max_windows=18, max_batch=18)
     reqs = _full_requests(16)
+    n = len(reqs)
+    assert [q["gk"]["max_length"] for q in reqs[-3:]] == [664, 1025, 2048]
     model.engine.encode(torch.cat([cases.model_pcm(cfg, 1, q["seed"]) for q in reqs]).cuda(), slot_begin=0)
     er = _engine_requests(reqs)
-    # Batch-1 calls on the default driver.  The one request whose max_length (664) needs 11 self-attention splits takes the graph
-    # driver: at these dimensions the dataflow megakernel's bounded wait for tagged data expires on that call (a limit of the uniform
-    # batch-1 path, observed at 11 splits x 12 heads = 132 units, not at 10 splits; the ragged call does not go through it).
-    want = [_single(model, layout, r, q, 0 if q["gk"]["max_length"] > 640 else 2) for r, q in enumerate(reqs)]
-    for pick in (list(range(0, 16, 2)), list(range(16))):
+    want = [_single(model, layout, r, q, 2) for r, q in enumerate(reqs)]
+    for pick in (list(range(0, n, 2)), list(range(n))):
         for k, got in zip(pick, model.engine.generate_ragged([er[k] for k in pick], layout)):
             assert got.shape[1] == reqs[k]["prompt"].shape[1] + 64
             _same(got.numpy(), want[k].numpy(), f"{len(pick)} requests, request {k} (P = {reqs[k]['prompt'].shape[1]})")
