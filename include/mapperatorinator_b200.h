@@ -280,6 +280,29 @@ int mb200_op_decode_attention(const float* q, const float* kv, int32_t slots, in
                               int32_t cur_len, int32_t prompt_len, const uint8_t* key_valid, int64_t key_valid_ld, int32_t max_length,
                               int32_t fixed_len, const int32_t* kv_src, int64_t kv_src_ld, const int32_t* ragged_cur_len,
                               const int32_t* ragged_max_length, int32_t form, float* out, void* cuda_stream);
+/* One output segment of mb200_op_gemv: stacked-weight columns [n_begin, n_end) go to out, row b at
+ * out + b * out_bs + (pos_stride ? (cur_len - 1) * pos_stride : 0) + (n - n_begin), as act(.) * alpha (+ the residual). */
+typedef struct mb200_gemv_seg {
+    float* out;
+    int64_t out_bs;
+    int64_t pos_stride;       /* != 0: write at the cache position of the token being processed */
+    int32_t n_begin, n_end;
+    float alpha;
+    int32_t act;              /* 0 none, 1 GELU (erf), 2 GELU (tanh), 3 SiLU */
+} mb200_gemv_seg;
+/* One weight-streaming GEMV phase of the token loop (decode.cu), through the engine's own launch_gemv:
+ *   out[b, n] = act(W[n, :] . X(x[b, :]) + bias[n]) * alpha + R[b, n],  b < B, n < N
+ * x [B rows of K at stride x_ld]; xmode 0 takes X = x, xmode 1 the LayerNorm X = LN(x) * ln_w + ln_b (K <= 1024); W [N rows of K
+ * at stride ldw]; bias [N] or null; R [B rows at stride r_ld] or null (it may be the output of segment 0: in-place residual).
+ * segs (host, 1 to 3) must tile [0, N) in order; cur_len >= 1 places the segments with a pos_stride.
+ * Ragged (ragged_cur_len and ragged_finished given, host int32 [n_req]): rows r and r + n_req share the state of request r % n_req;
+ * a positional segment writes row b at its own cur_len - 1, and not at all once the row has finished.
+ * form: 0 the per-phase kernel, 1 the barrier megakernel's phase body (B <= 2, not ragged).
+ * All pointers except segs / ragged_* are DEVICE.  Synchronises the stream before it returns. */
+int mb200_op_gemv(const float* x, int64_t x_ld, int32_t B, int32_t K, int32_t xmode, const float* ln_w, const float* ln_b, float eps,
+                  const float* W, int64_t ldw, int32_t N, const float* bias, const float* R, int64_t r_ld, const mb200_gemv_seg* segs,
+                  int32_t nseg, int32_t cur_len, const int32_t* ragged_cur_len, const int32_t* ragged_finished, int32_t n_req,
+                  int32_t form, void* cuda_stream);
 /* Tuning / tests: tensor-core (wgmma, 3xTF32) flash attention on or off, and the minimum number of queries for which it is used
    (attention_tc.cu; replaces the SIMT kernel for the encoder self-attention of HF modeling_whisper.py:286-358 and the DiT band of
    osu_diffusion/utils/models.py:145-151). */

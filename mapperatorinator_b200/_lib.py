@@ -41,6 +41,11 @@ class DitConfigC(C.Structure):
                 ("t_freq_dim", C.c_int32), ("max_seq_len", C.c_int32), ("max_batch", C.c_int32)]
 
 
+class GemvSegC(C.Structure):
+    _fields_ = [("out", C.c_void_p), ("out_bs", C.c_int64), ("pos_stride", C.c_int64), ("n_begin", C.c_int32), ("n_end", C.c_int32),
+                ("alpha", C.c_float), ("act", C.c_int32)]
+
+
 class DitMaskC(C.Structure):
     _fields_ = [("mask_mode", C.c_int32), ("band", C.c_int32), ("dense_mask", C.c_void_p)]
 
@@ -56,7 +61,7 @@ ABI_SYMBOLS = [
     "mb200_dit_sample_loop", "mb200_dit_set_option", "mb200_dit_set_sliders", "mb200_dit_apply_sliders",
     "mb200_launch_count", "mb200_model_set_option", "mb200_model_profile_step", "mb200_model_read_trace", "mb200_model_mega_stats", "mb200_model_logits_chain",
     "mb200_model_beam_step",
-    "mb200_op_gemm", "mb200_op_gemm_tc", "mb200_set_tensor_cores", "mb200_op_layernorm", "mb200_op_attention", "mb200_op_decode_attention", "mb200_set_attention_tc", "mb200_audio_out_frames", "mb200_audio_ingest",
+    "mb200_op_gemm", "mb200_op_gemm_tc", "mb200_set_tensor_cores", "mb200_op_layernorm", "mb200_op_attention", "mb200_op_decode_attention", "mb200_op_gemv", "mb200_set_attention_tc", "mb200_audio_out_frames", "mb200_audio_ingest",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -112,6 +117,8 @@ def load() -> C.CDLL:
     lib.mb200_op_attention.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, f32, i32, i32, vp, i32, vp, vp]
     lib.mb200_set_attention_tc.argtypes = [i32, i32]
     lib.mb200_op_decode_attention.argtypes = [vp, vp, i32, i32, i32, i32, vp, i32, i32, vp, i64, i32, i32, vp, i64, vp, vp, i32, vp, vp]
+    lib.mb200_op_gemv.argtypes = [vp, i64, i32, i32, i32, vp, vp, f32, vp, i64, i32, vp, vp, i64, C.POINTER(GemvSegC), i32, i32, vp, vp,
+                                  i32, i32, vp]
     lib.mb200_audio_out_frames.argtypes = [i64, i32, i32]
     lib.mb200_audio_out_frames.restype = i64
     lib.mb200_audio_ingest.argtypes = [vp, i64, i32, i32, i32, i32, vp, vp, vp]

@@ -190,6 +190,60 @@ extern "C" int mb200_op_decode_attention(const float* q, const float* kv, int32_
     return 0;
 }
 
+// One GEMV phase through launch_gemv, with the GemvParams a token step builds and the call state (GenState, RowStates) owned here.
+extern "C" int mb200_op_gemv(const float* x, int64_t x_ld, int32_t B, int32_t K, int32_t xmode, const float* ln_w, const float* ln_b,
+                             float eps, const float* W, int64_t ldw, int32_t N, const float* bias, const float* R, int64_t r_ld,
+                             const mb200_gemv_seg* segs, int32_t nseg, int32_t cur_len, const int32_t* ragged_cur_len,
+                             const int32_t* ragged_finished, int32_t n_req, int32_t form, void* stream) {
+    MB_REQUIRE(x && W && segs, "null argument");
+    MB_REQUIRE(B >= 1 && N >= 1 && K >= 4, "need B >= 1, N >= 1, K >= 4");
+    MB_REQUIRE(x_ld >= K && ldw >= K && (!R || r_ld >= N), "a row stride is shorter than its row");
+    MB_REQUIRE(reinterpret_cast<uintptr_t>(x) % 16 == 0 && reinterpret_cast<uintptr_t>(W) % 16 == 0, "x and W are read as float4");
+    MB_REQUIRE(xmode == X_PLAIN || xmode == X_LAYERNORM, "unknown input mode");
+    MB_REQUIRE(xmode != X_LAYERNORM || (ln_w && ln_b), "a LayerNorm input needs its weight and bias");
+    MB_REQUIRE(nseg >= 1 && nseg <= 3, "1 to 3 output segments");
+    const bool ragged = ragged_cur_len != nullptr;
+    MB_REQUIRE(ragged == (ragged_finished != nullptr), "a ragged call gives both per-row cur_len and finished");
+    bool positional = false;
+    GemvParams g{};
+    g.xmode = xmode; g.x = x; g.x_ld = x_ld; g.ln_w = ln_w; g.ln_b = ln_b; g.eps = eps;
+    g.W = W; g.ldw = ldw; g.bias = bias; g.K = K; g.N = N; g.B = B; g.R = R; g.r_ld = r_ld;
+    g.nseg = nseg;
+    for (int i = 0; i < nseg; ++i) {
+        const mb200_gemv_seg& s = segs[i];
+        MB_REQUIRE(s.out, "a segment without an output");
+        MB_REQUIRE(s.n_begin == (i ? segs[i - 1].n_end : 0) && s.n_begin < s.n_end && (i + 1 < nseg || s.n_end == N),
+                   "the segments must tile [0, N) in order");
+        MB_REQUIRE(s.act >= ACT_NONE && s.act <= ACT_SILU, "unknown activation");
+        positional = positional || s.pos_stride != 0;
+        g.seg[i] = GemvSeg{s.out, s.out_bs, s.pos_stride, s.n_begin, s.n_end, s.alpha, s.act};
+    }
+    GenState gs{};
+    std::vector<RowState> rs;
+    if (ragged) {
+        MB_REQUIRE(n_req >= 1 && n_req <= B, "need 1 <= n_req <= B");
+        gs.n_req = n_req;
+        rs.resize(n_req);
+        for (int r = 0; r < n_req; ++r) {
+            MB_REQUIRE(ragged_cur_len[r] >= 1, "need cur_len >= 1 in every row");
+            MB_REQUIRE(ragged_finished[r] == 0 || ragged_finished[r] == 1, "finished is 0 or 1");
+            rs[r].cur_len = ragged_cur_len[r]; rs[r].finished = ragged_finished[r];
+        }
+    } else {
+        MB_REQUIRE(!positional || cur_len >= 1, "a segment that writes at the cache position needs cur_len >= 1");
+        gs.cur_len = cur_len;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    static OpScratch op_state;
+    OP_TRY(op_state.ensure(sizeof(GenState) + rs.size() * sizeof(RowState)));
+    MB_CUDA_CHECK(cudaMemcpyAsync(op_state.p, &gs, sizeof(GenState), cudaMemcpyHostToDevice, st));
+    if (ragged) MB_CUDA_CHECK(cudaMemcpyAsync(reinterpret_cast<GenState*>(op_state.p) + 1, rs.data(), rs.size() * sizeof(RowState), cudaMemcpyHostToDevice, st));
+    g.st = reinterpret_cast<const GenState*>(op_state.p);
+    const int rc = launch_gemv(g, st, false, ragged, form);     // also where the shape requirements of the kernels are checked
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));      // the host-side state above goes out of scope
+    return rc;
+}
+
 // tuning / tests: minimum query count for the tensor-core attention path (0 disables it)
 extern "C" int mb200_set_attention_tc(int32_t enabled, int32_t min_queries) {
     g_attn_tc_enabled = enabled; g_attn_tc_min_t = min_queries;

@@ -9,6 +9,7 @@
 //
 // The GEMVs are weight-streaming (HBM-bound): one warp per output row, float4 coalesced reads of the [N, K] row-major
 // weight, activations for up to 8 batch rows staged in shared memory, fp32 accumulation in a fixed order.
+#include <algorithm>
 #include <cstdlib>
 #include "common.cuh"
 #include "kernels.h"
@@ -33,6 +34,34 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(GemvParams p) {
             gemv_row<NB, true, RAGGED>(p, n, p.W + (long long)n * p.ldw, xs, b0, lane, cur_pos);
         __syncthreads();
     }
+}
+
+// The barrier megakernel's GEMV phase (decode_mega.cu) as a kernel of its own: the megakernel's 512 threads stage the activations, CTA c
+// holds weight rows [c * rpc, (c + 1) * rpc), rpc = ceil(N / grid), in shared memory (the megakernel streams them there with bulk
+// copies; plain loads here) and warp w runs gemv_row on rows r0 + w, r0 + w + 16, ...  Only the kernel-level tests launch it, to hold
+// the two forms to the same bits.
+constexpr int MEGA_GEMV_THREADS = SAMPLE_THREADS;      // decode_mega.cu's MEGA_THREADS
+
+template <int NB>
+__global__ void __launch_bounds__(MEGA_GEMV_THREADS) gemv_mega_body_kernel(GemvParams p) {
+    extern __shared__ __align__(16) float sm[];   // [rpc][K] weight rows, [NB][K] activations, 32 floats of LayerNorm reduction scratch
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    pdl_launch_dependents();
+    pdl_wait();
+    const int rpc = (p.N + (int)gridDim.x - 1) / (int)gridDim.x;
+    const int r0 = min(p.N, (int)blockIdx.x * rpc), r1 = min(p.N, r0 + rpc);
+    const int K4 = p.K >> 2;
+    float* wbuf = sm;
+    float* xs = sm + (long long)rpc * p.K;
+    for (int e = tid; e < (r1 - r0) * K4; e += MEGA_GEMV_THREADS) {
+        const int r = e / K4, c = e - r * K4;
+        reinterpret_cast<float4*>(wbuf)[e] = __ldg(reinterpret_cast<const float4*>(p.W + (long long)(r0 + r) * p.ldw) + c);
+    }
+    gemv_stage_x<NB, MEGA_GEMV_THREADS>(p, 0, xs, xs + NB * p.K, tid);
+    __syncthreads();
+    const int cur_pos = p.st ? p.st->cur_len - 1 : 0;
+    for (int n = r0 + warp; n < r1; n += MEGA_GEMV_THREADS / 32)
+        gemv_row<NB, false>(p, n, wbuf + (long long)(n - r0) * p.K, xs, 0, lane, cur_pos);
 }
 
 template <int KMAX, bool TABLE = false>
@@ -166,10 +195,29 @@ int launch_with_attrs(Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_
 
 }  // namespace
 
-int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged) {
-    MB_REQUIRE(p.K % 4 == 0 && p.ldw % 4 == 0, "GEMV K / ldw must be multiples of 4");
+int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged, int form) {
+    MB_REQUIRE(p.K % 4 == 0 && p.ldw % 4 == 0 && p.x_ld % 4 == 0, "GEMV K / ldw / x_ld must be multiples of 4");
     MB_REQUIRE(p.xmode != X_LAYERNORM || p.K <= 1024, "fused LayerNorm prologue supports K <= 1024");
+    MB_REQUIRE(form == GEMV_FORM_KERNEL || form == GEMV_FORM_MEGA, "unknown GEMV form");
+    MB_REQUIRE(form != GEMV_FORM_MEGA || (!ragged && p.B <= 2), "the megakernel's GEMV body runs 1 or 2 rows, not ragged");
     if (p.B <= 0 || p.N <= 0) return 0;
+    if (form == GEMV_FORM_MEGA) {
+        // a 132-CTA grid like the megakernel's on an H100, more CTAs when that many rows per CTA would not fit shared memory
+        const size_t limit = 200 * 1024, fixed = ((size_t)p.B * p.K + 32) * sizeof(float), row = (size_t)p.K * sizeof(float);
+        MB_REQUIRE(fixed + row <= limit, "GEMV activation tile does not fit shared memory");
+        const int rpc = (int)std::min<size_t>((p.N + 131) / 132, (limit - fixed) / row);
+        static bool mega_configured = false;
+        if (!mega_configured) {
+            MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_mega_body_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit));
+            MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_mega_body_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit));
+            mega_configured = true;
+        }
+        const dim3 grid((p.N + rpc - 1) / rpc);       // the kernel's ceil(N / grid) is at most rpc
+        const size_t smem = fixed + rpc * row;
+        g_prof_class = 0;
+        return p.B == 1 ? launch_with_attrs(gemv_mega_body_kernel<1>, grid, dim3(MEGA_GEMV_THREADS), smem, stream, pdl, p)
+                        : launch_with_attrs(gemv_mega_body_kernel<2>, grid, dim3(MEGA_GEMV_THREADS), smem, stream, pdl, p);
+    }
     int nb = p.B >= 8 ? 8 : (p.B > 4 ? 8 : (p.B > 2 ? 4 : p.B));
     const size_t smem = ((size_t)nb * p.K + 32) * sizeof(float);
     const int blocks = (p.N + GEMV_WARPS - 1) / GEMV_WARPS;

@@ -231,8 +231,12 @@ struct GemvParams {
     const float* R; long long r_ld;                 // residual rows for segment 0 (null = none)
     const GenState* st;
 };
+// Which kernel body runs the rows.  KERNEL is the per-phase gemv_kernel (4 warps, weights read from global memory); MEGA is the barrier
+// megakernel's phase body (16 warps, each CTA's weight rows copied to shared memory first; B <= 2, not ragged), which the kernel-level
+// tests compare with KERNEL bit for bit.
+enum GemvForm : int { GEMV_FORM_KERNEL = 0, GEMV_FORM_MEGA = 1 };
 // ragged: p.st heads a ragged state; segments with pos_stride write row b at ITS cache position, and not at all once it has finished
-int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged = false);
+int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged = false, int form = GEMV_FORM_KERNEL);
 
 struct DecAttnParams {
     const float* q; long long q_ld;                 // [rows, d_model], already scaled

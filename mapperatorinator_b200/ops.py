@@ -1,6 +1,7 @@
 """Kernel-level wrappers over the C ABI (`mb200_op_*`) for parity tests; operands are CUDA torch tensors."""
 from __future__ import annotations
 
+from dataclasses import dataclass
 from typing import Optional
 
 import torch
@@ -97,4 +98,55 @@ def decode_attention(q, kv, heads, *, row_slot=None, cur_len=0, prompt_len=0, ke
                                              int(fixed_len), _ptr(kv_src), kv_src.shape[1] if kv_src is not None else 0,
                                              None if rc is None else C.cast(rc, C.c_void_p), None if rm is None else C.cast(rm, C.c_void_p),
                                              DECODE_ATTENTION_FORMS[form], _ptr(out), _stream()))
+    return out
+
+
+@dataclass
+class GemvSegment:
+    """Columns [n_begin, n_end) of a GEMV's stacked weight, written from the data pointer of `out` (any float32 CUDA view): row b at
+    b * out_bs + (cur_len - 1) * pos_stride + (n - n_begin), the middle term only for a segment that writes at the cache position."""
+    out: torch.Tensor
+    n_begin: int
+    n_end: int
+    out_bs: int
+    pos_stride: int = 0
+    act: str = "none"
+    alpha: float = 1.0
+
+
+GEMV_FORMS = {"kernel": 0, "mega": 1}
+
+
+def gemv(x, w, bias=None, *, ln_weight=None, ln_bias=None, eps=1e-5, xmode=None, residual=None, act="none", alpha=1.0, out=None,
+         segments=None, cur_len=0, ragged_cur_len=None, ragged_finished=None, n_req=None, form="kernel"):
+    """One weight-streaming GEMV phase of the token loop (`mb200_op_gemv`): act(w @ X(x[b]) + bias) * alpha + residual[b].
+
+    x (B, K) and w (N, K) may be row-strided views (unit column stride); X is the fused LayerNorm when ln_weight / ln_bias are given
+    (xmode "layernorm", or force either mode by name).  Without `segments` the output is one segment over [0, N) into `out` (allocated
+    (B, N) when not given; it may be `residual` itself) and is returned.  `segments` (GemvSegment, 1 to 3) route the columns instead,
+    positional ones at `cur_len` (or per request: ragged_cur_len / ragged_finished with rows r and r + n_req sharing request r).
+    form "kernel" is the per-phase kernel, "mega" the barrier megakernel's phase body."""
+    import ctypes as C
+    lib = _lib.load()
+    for t in (x, w, bias, ln_weight, ln_bias, residual, out):
+        assert t is None or (t.is_cuda and t.dtype == torch.float32 and t.stride(-1) == 1)
+    B, K = x.shape
+    N = w.shape[0]
+    if xmode is None:
+        xmode = "layernorm" if ln_weight is not None else "plain"
+    if segments is None:
+        if out is None:
+            out = torch.empty(B, N, device=x.device, dtype=torch.float32)
+        segments = [GemvSegment(out, 0, N, out.stride(0), 0, act, alpha)]
+    segs = (_lib.GemvSegC * len(segments))(*[_lib.GemvSegC(s.out.data_ptr(), int(s.out_bs), int(s.pos_stride), int(s.n_begin), int(s.n_end),
+                                                             float(s.alpha), ACT[s.act]) for s in segments])
+    rc = rf = None
+    if ragged_cur_len is not None:
+        n_req = len(ragged_cur_len) if n_req is None else n_req
+        rc = (C.c_int32 * n_req)(*[int(v) for v in ragged_cur_len])
+        rf = (C.c_int32 * n_req)(*[int(v) for v in ragged_finished])
+    _lib.check(lib.mb200_op_gemv(_ptr(x), x.stride(0), B, K, {"plain": 0, "layernorm": 1}[xmode], _ptr(ln_weight), _ptr(ln_bias), float(eps),
+                                 _ptr(w), w.stride(0), N, _ptr(bias), _ptr(residual), residual.stride(0) if residual is not None else 0,
+                                 segs, len(segments), int(cur_len), None if rc is None else C.cast(rc, C.c_void_p),
+                                 None if rf is None else C.cast(rf, C.c_void_p), int(n_req or 0), GEMV_FORMS[form], _stream()))
     return out
