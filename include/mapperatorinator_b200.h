@@ -139,6 +139,31 @@ int mb200_model_generate_ragged(mb200_model* m, int32_t n_req, const int32_t* sl
                                 const int64_t* neg_prompt, const uint8_t* vflags, const mb200_generate_params* params,
                                 int64_t* out_ids, int32_t out_ld, int32_t* out_len, void* cuda_stream);
 
+/* Decode stream: continuous batching in the token loop.  A ragged token loop with a fixed row capacity: requests are admitted into free
+ * rows between token steps and handed back as soon as they finish, and their rows are reused.  Every request's ids are bit-identical to
+ * its own batch-1 mb200_model_generate call, whatever step it joins at, whatever the other rows do and whatever its row held before.
+ * One stream per engine: while it is open, generate / generate_beams / generate_ragged / forward_logits / score_tokens refuse;
+ * mb200_model_encode into slots no live row reads stays allowed.  Beam search does not run in a stream.
+ *   open:  capacity requests (2 * capacity decoder rows when use_cfg: every request guided, or none), each with max_length <= the
+ *          max_length cap.  Captures the stream's token-step graph the first time this shape is seen; synchronises the stream.
+ *   admit: n requests, arguments as for mb200_model_generate_ragged (HOST memory), into the lowest free rows (rows_out[n]).  Stages
+ *          the rows and queues their prompt scan, batch-1 prefill and first-token selection with no host wait.  Rejected before
+ *          anything is launched: fewer free rows than n, prompt_len >= max_length, max_length above the cap, a guidance mismatch
+ *          with the stream, token ids out of range; the stream stays usable.
+ *   run:   one burst of *steps token steps (short while `waiting` requests wait for a row, else up to 16), then the rows that
+ *          finished in it: done_rows[n_done], done_len[n_done] (capacity entries each).  Synchronises the stream.
+ *   take:  copies a finished row's ids (prompt + generated, done_len of them) to out_ids (HOST, out_ld wide) and frees the row.
+ *   close: frees the stream; the engine's other token-loop calls work again. */
+typedef struct mb200_stream mb200_stream;
+int mb200_stream_open(mb200_model* m, int32_t capacity, int32_t use_cfg, int32_t max_length, mb200_stream** out, void* cuda_stream);
+int mb200_stream_admit(mb200_stream* s, int32_t n, const int32_t* slots, const int64_t* prompt, const int32_t* prompt_off,
+                       const int64_t* neg_prompt, const uint8_t* vflags, const mb200_generate_params* params, int32_t* rows_out,
+                       void* cuda_stream);
+int mb200_stream_run(mb200_stream* s, int32_t waiting, int32_t* done_rows, int32_t* done_len, int32_t* n_done, int32_t* steps,
+                     void* cuda_stream);
+int mb200_stream_take(mb200_stream* s, int32_t row, int64_t* out_ids, int32_t out_ld, void* cuda_stream);
+void mb200_stream_close(mb200_stream* s);
+
 /* Mapperatorinator.forward teacher-forced logits (server.model_forward, server.py:159-181), no CFG mixing.
  * ids: HOST int64 [batch, len]; mask HOST uint8; logits_out: DEVICE f32 [batch, len, vocab_size_out]. */
 int mb200_model_forward_logits(mb200_model* m, const int32_t* slots, int32_t batch, const int64_t* ids, const uint8_t* mask,

@@ -56,6 +56,7 @@ ABI_SYMBOLS = [
     "mb200_mel_create", "mb200_mel_destroy", "mb200_mel_forward",
     "mb200_model_create", "mb200_model_destroy", "mb200_model_set_weight", "mb200_model_finalize", "mb200_model_encode",
     "mb200_model_generate", "mb200_model_generate_beams", "mb200_model_generate_ragged", "mb200_model_forward_logits",
+    "mb200_stream_open", "mb200_stream_admit", "mb200_stream_run", "mb200_stream_take", "mb200_stream_close",
     "mb200_model_score_tokens",
     "mb200_dit_create", "mb200_dit_destroy", "mb200_dit_set_weight", "mb200_dit_finalize", "mb200_dit_forward_with_cfg",
     "mb200_dit_sample_loop", "mb200_dit_set_option", "mb200_dit_set_sliders", "mb200_dit_apply_sliders",
@@ -91,6 +92,11 @@ def load() -> C.CDLL:
     lib.mb200_model_generate_beams.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp, vp, C.POINTER(GenerateParamsC), i32, i64, vp,
                                                C.POINTER(i32), vp, vp]
     lib.mb200_model_generate_ragged.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, i32, vp, vp]
+    lib.mb200_stream_open.argtypes = [vp, i32, i32, i32, C.POINTER(vp), vp]
+    lib.mb200_stream_admit.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.mb200_stream_run.argtypes = [vp, i32, vp, vp, C.POINTER(i32), C.POINTER(i32), vp]
+    lib.mb200_stream_take.argtypes = [vp, i32, vp, i32, vp]
+    lib.mb200_stream_close.argtypes = [vp]; lib.mb200_stream_close.restype = None
     lib.mb200_model_forward_logits.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, vp]
     lib.mb200_model_score_tokens.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, vp, vp, vp, vp]
     lib.mb200_model_set_option.argtypes = [vp, C.c_char_p, i32]

@@ -108,6 +108,8 @@ __global__ void __launch_bounds__(128, 4) decode_attention_ragged_kernel(DecAttn
     pdl_wait();
     const int s = blockIdx.x, h = blockIdx.y, r = blockIdx.z;
     const RowState* rs = ragged_rows(p.st) + r % p.st->n_req;
+    // a finished row (or a vacant stream row) appends nothing and its output is never read: no keys, no ticket
+    if (rs->finished) return;
     const int L = rs->cur_len;
     const int S = self_splits(rs->max_length);
     if (s >= S) return;                                // uniform across the CTA
@@ -130,6 +132,12 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleParams p) 
     sample_body<SAMPLE_THREADS, RAGGED>(p, blockIdx.x, sm);
 }
 
+// the ragged selection of the listed rows only (decode stream admissions): CTA i runs row rows[i] at whatever step that row is at
+__global__ void __launch_bounds__(SAMPLE_THREADS) sample_rows_kernel(SampleParams p, const int* rows) {
+    __shared__ SampleSmem sm;
+    sample_body<SAMPLE_THREADS, true>(p, rows[blockIdx.x], sm);
+}
+
 __global__ void prompt_scan_kernel(const long long* ids, long long ids_ld, int P, const unsigned char* vflags, int ts_start, int ts_end,
                                    int* last_ts) {
     const int b = blockIdx.x;
@@ -144,8 +152,8 @@ __global__ void prompt_scan_kernel(const long long* ids, long long ids_ld, int P
 }
 
 __global__ void prompt_scan_ragged_kernel(const long long* ids, long long ids_ld, const GenState* st, const unsigned char* vflags, long long vflags_ld,
-                                          int ts_start, int ts_end, int* last_ts) {
-    const int b = blockIdx.x;
+                                          int ts_start, int ts_end, int* last_ts, const int* rows) {
+    const int b = rows ? rows[blockIdx.x] : blockIdx.x;
     if (threadIdx.x != 0) return;
     const int P = ragged_rows(st)[b].prompt_len;
     const unsigned char* vf = vflags + b * vflags_ld;
@@ -299,6 +307,15 @@ int launch_sample(const SampleParams& p, int B, cudaStream_t stream, bool pdl, b
     return launch_with_attrs(sample_kernel<false>, dim3(B), dim3(SAMPLE_THREADS), 0, stream, pdl, p);
 }
 
+int launch_sample_rows(const SampleParams& p, const int* rows, int n, cudaStream_t stream) {
+    if (n <= 0) return 0;
+    g_prof_class = 2;
+    sample_rows_kernel<<<n, SAMPLE_THREADS, 0, stream>>>(p, rows);
+    MB_LAUNCH_CHECK();
+    ++g_launch_count;
+    return 0;
+}
+
 int launch_prompt_scan(const long long* ids, long long ids_ld, int B, int P, const unsigned char* vflags, int ts_start, int ts_end,
                        int* last_ts, cudaStream_t stream) {
     prompt_scan_kernel<<<B, 32, 0, stream>>>(ids, ids_ld, P, vflags, ts_start, ts_end, last_ts);
@@ -307,9 +324,10 @@ int launch_prompt_scan(const long long* ids, long long ids_ld, int B, int P, con
     return 0;
 }
 
-int launch_prompt_scan_ragged(const long long* ids, long long ids_ld, int B, const GenState* st, const unsigned char* vflags, long long vflags_ld,
-                              int ts_start, int ts_end, int* last_ts, cudaStream_t stream) {
-    prompt_scan_ragged_kernel<<<B, 32, 0, stream>>>(ids, ids_ld, st, vflags, vflags_ld, ts_start, ts_end, last_ts);
+int launch_prompt_scan_ragged(const long long* ids, long long ids_ld, int n, const GenState* st, const unsigned char* vflags, long long vflags_ld,
+                              int ts_start, int ts_end, int* last_ts, cudaStream_t stream, const int* rows) {
+    if (n <= 0) return 0;
+    prompt_scan_ragged_kernel<<<n, 32, 0, stream>>>(ids, ids_ld, st, vflags, vflags_ld, ts_start, ts_end, last_ts, rows);
     MB_LAUNCH_CHECK();
     ++g_launch_count;
     return 0;

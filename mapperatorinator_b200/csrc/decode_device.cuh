@@ -1008,8 +1008,9 @@ static __device__ __forceinline__ void logits_chain(const SampleParams& p, int b
 // so this is about code size and register pressure of the caller, not about the 32 KB L1.5 instruction cache.)
 // Returns after the "last CTA" bookkeeping; the caller decides how the grid synchronises afterwards.
 // NT = threads of the calling CTA (512 in the per-phase kernel and the barrier megakernel, 256 in the dataflow megakernel).
-// RAGGED: lengths, limits and the finished flag are row b's own (ragged_rows(st)[b]); the draw uses row index 0 in its counter, as the
-// row's batch-1 call would; a finished row is frozen (nothing appended, its last embedding re-issued so the residual stream stays put).
+// RAGGED: lengths, limits, the finished flag, the step counter and the look-back flag are row b's own (ragged_rows(st)[b]); the draw
+// uses the row's step and row index 0 in its counter, as the row's batch-1 call would; a finished row is frozen (nothing appended, its
+// last embedding re-issued so the residual stream stays put).
 template <int NT, bool RAGGED = false>
 static __device__ __noinline__ void sample_body(const SampleParams& p, int b, SampleSmem& sm) {
     float* s = sm.s;
@@ -1023,7 +1024,7 @@ static __device__ __noinline__ void sample_body(const SampleParams& p, int b, Sa
     const int L = ld_state(RAGGED ? &rs->cur_len : &st->cur_len);
     const int st_prompt_len = ld_state(RAGGED ? &rs->prompt_len : &st->prompt_len);
     const int st_min_new = ld_state(RAGGED ? &rs->min_new_tokens : &st->min_new_tokens);
-    const int st_step = ld_state(&st->step), st_has_last = ld_state(&st->has_last_scores);
+    const int st_step = ld_state(RAGGED ? &rs->step : &st->step), st_has_last = ld_state(RAGGED ? &rs->has_last_scores : &st->has_last_scores);
     const int st_max_length = ld_state(RAGGED ? &rs->max_length : &st->max_length);
     long long* ids_row = p.ids + (long long)b * c.ids_ld;
     const bool suppress_eos = st_min_new > 0 && (L - st_prompt_len) < st_min_new;
@@ -1185,7 +1186,9 @@ static __device__ __noinline__ void sample_body(const SampleParams& p, int b, Sa
         bool fin = was_finished || ((row_vflags<RAGGED>(p, c, b)[tok] & VF_EOS) != 0) || (L + 1 >= st_max_length);
         if (RAGGED) {
             rs->cur_len = L + 1;
-            if (fin) { rs->finished = 1; atomicAdd(&st->n_finished, 1); }
+            rs->step = st_step + 1;
+            rs->has_last_scores = 1;
+            if (fin) rs->finished = 1;
         } else if (fin && !was_finished) { p.finished[b] = 1; atomicAdd(&st->n_finished, 1); }
         // MonotonicTimeShift state (logit_processors.py:149-166): last time shift after the last SOS-type token
         const unsigned char fl = row_vflags<RAGGED>(p, c, b)[tok];
@@ -1219,17 +1222,29 @@ static __device__ __noinline__ void sample_body(const SampleParams& p, int b, Sa
     if (tid == 0) {
         // Last row to arrive publishes the next token's header.  Dataflow megakernel: the tagged header goes out FIRST (its consumers
         // synchronise on the tag, not on the fences); the plain state for the host / the per-phase kernels follows.
-        if (B > 1) __threadfence();                    // this row's n_finished update before its ticket
-        if (atomicAdd(&st->ticket, 1) == B - 1) {
-            const int fin_all = (ld_state(&st->n_finished) >= B || (!RAGGED && L + 1 >= st_max_length)) ? 1 : 0;
+        // RAGGED: one CTA per row of the launch — every row of the state, or the rows of an admission's list
+        const int n_cta = RAGGED ? (int)gridDim.x : B;
+        if (n_cta > 1) __threadfence();                // this row's finished update before its ticket
+        if (atomicAdd(&st->ticket, 1) == n_cta - 1) {
+            int fin_all;
+            if (RAGGED) {      // all rows of the state, launched or not; a vacant stream row is a finished row
+                fin_all = 1;
+                const int n = ld_state(&st->n_req);
+                for (int r = 0; r < n; ++r)
+                    if (!ld_state(&ragged_rows(st)[r].finished)) fin_all = 0;
+            } else {
+                fin_all = (ld_state(&st->n_finished) >= B || L + 1 >= st_max_length) ? 1 : 0;
+            }
             if (p.ll_hdr) {        // token header of the dataflow megakernel: next cur_len, all-finished flag
                 ll_store(p.ll_hdr + 0, __int_as_float(L + 1), p.ll_out_tag);
                 ll_store(p.ll_hdr + 1, __int_as_float(fin_all), p.ll_out_tag);
             }
             st->ticket = 0;
             if (!RAGGED) st->cur_len = L + 1;
-            st->step = st_step + 1;
-            st->has_last_scores = 1;
+            if (!RAGGED) {     // a ragged row advanced its own step above
+                st->step = st_step + 1;
+                st->has_last_scores = 1;
+            }
             if (fin_all) st->all_finished = 1;
             __threadfence();
         }

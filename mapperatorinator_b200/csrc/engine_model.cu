@@ -2,6 +2,7 @@
 // prefill, CUDA-graph token loop.  Mirrors what `server.model_generate` drives through HF `generate`
 // (osuT5/osuT5/inference/server.py:83-156) — see include/mapperatorinator_b200.h for the boundary.
 #include <algorithm>
+#include <climits>
 #include <cstring>
 #include <functional>
 #include <map>
@@ -102,6 +103,7 @@ struct mb200_model {
     AttnCtx attn;                       // tensor-core attention scratch of the encoder (head-major tf32 copies of q | k | v^T)
     GemmCtx gemm;                       // this engine's GEMM scratch: split-K planes, tf32 activation copies, weight mirrors, error flag
     DevBuf s_logits;                    // token scoring: one chunk of vocabulary-projection rows [<= SCORE_CHUNK_ROWS, V]
+    mb200_stream* live_stream = nullptr; // the open decode stream: it owns g_state, g_ids and the logits rows until closed
 
     int d() const { return cfg.d_model; }
     int Ts() const { return cfg.src_seq_len / 2; }
@@ -341,11 +343,14 @@ extern "C" int mb200_model_finalize(mb200_model* m) {
     MB_TRY(m->g_prefill_ids.ensure((size_t)m->max_rows * c.tgt_seq_len * sizeof(long long)));
     MB_TRY(m->g_keyvalid.ensure((size_t)m->max_rows * c.tgt_seq_len));
     MB_TRY(m->g_leftpad.ensure(m->max_rows * sizeof(int)));
-    MB_TRY(m->g_rowslot.ensure((size_t)3 * m->max_rows * sizeof(int)));   // [max_rows] decode rows, then one (slot, slot) pair per request for ragged prefills
+    // [max_rows] decode rows, then one (slot, slot) pair per request for ragged prefills, then the row list of a stream admission
+    MB_TRY(m->g_rowslot.ensure((size_t)4 * m->max_rows * sizeof(int)));
     MB_TRY(m->g_finished.ensure(m->max_rows));
     {
         const size_t tgt = (size_t)m->max_rows * c.tgt_seq_len;
         m->h_stage_bytes = tgt * 8 * 2 + tgt + (size_t)2 * m->max_rows * 4 + c.vocab_size_in + sizeof(GenState) + sizeof(SampleConfig) + 8 * 16;
+        // a stream admission of up to max_rows requests: per row a flag row, RowState, SampleConfig, slot entries and their alignment
+        m->h_stage_bytes += (size_t)m->max_rows * (c.vocab_size_in + sizeof(RowState) + sizeof(SampleConfig) + 16 + 5 * 16) + 16;
         MB_CUDA_CHECK(cudaMallocHost(&m->h_stage, m->h_stage_bytes));
         MB_CUDA_CHECK(cudaEventCreateWithFlags(&m->stage_ev, cudaEventDisableTiming));
     }
@@ -892,6 +897,7 @@ extern "C" int mb200_model_generate(mb200_model* m, const int32_t* slots, int32_
                                     int32_t P, const int64_t* neg_prompt, const uint8_t* neg_mask, const uint8_t* vflags,
                                     const mb200_generate_params* gp, int64_t* out_ids, int32_t* out_len, void* stream) {
     MB_REQUIRE(m && m->finalized, "model not finalized");
+    MB_REQUIRE(!m->live_stream, "a decode stream is open on this engine: close it first");
     MB_REQUIRE(slots && prompt && vflags && gp && out_ids && out_len, "null argument");
     const auto& c = m->cfg;
     cudaStream_t st = (cudaStream_t)stream;
@@ -1080,24 +1086,304 @@ extern "C" int mb200_model_generate(mb200_model* m, const int32_t* slots, int32_
 }
 
 // =====================================================================================================================
+// Decode stream: a ragged token loop with a fixed row capacity N.  Requests are admitted into free rows between token steps and handed
+// back as soon as they finish; each row's ids are bit-identical to its own batch-1 mb200_model_generate call, whatever step it joins at,
+// whatever its neighbours do, and whatever the row held before.  Row r's state is its RowState (own length, plan, step counter and
+// look-back flag), its SampleConfig and flag row, and its cache rows r (and N + r under classifier-free guidance).  A vacant row is a
+// finished row: the step skips its self attention and leaves its cache and ids alone.  The ragged call below is one such stream that
+// admits everything at once.  The two megakernels stay uniform (rows <= 2).
+// =====================================================================================================================
+struct mb200_stream {
+    mb200_model* m = nullptr;
+    int N = 0, rows = 0, cap = 0;
+    bool use_cfg = false;
+    cudaGraphExec_t step = nullptr;          // owned by m->graphs
+    long long step_nodes = 0;
+    enum : int { FREE = 0, LIVE = 1, DONE = 2 };
+    std::vector<int> status;                 // host view of each row
+    std::vector<int> prompt_len, max_length, first_poll, selections;
+    std::vector<int> done_len;               // DONE rows: final length
+    RowState* h_rows = nullptr;              // pinned [N]: the rows' device state read back after each burst
+};
+
+namespace {
+
+void stream_release(mb200_stream* s) {
+    if (s->h_rows) cudaFreeHost(s->h_rows);
+    s->h_rows = nullptr;
+}
+
+// Fixes the shape (capacity N, guidance, max_length cap), captures the ragged step graph of (rows, N, self_splits(cap)) if this engine
+// has none yet, and marks every row vacant.  Synchronises `st`.
+int stream_open(mb200_model* m, mb200_stream* s, int N, bool use_cfg, int cap, cudaStream_t st) {
+    const auto& c = m->cfg;
+    const int rows = use_cfg ? 2 * N : N;
+    MB_REQUIRE(N >= 1 && rows <= m->max_rows, "stream capacity exceeds max_batch (rows double under classifier-free guidance)");
+    MB_REQUIRE(cap >= 2 && cap <= c.tgt_seq_len, "need 2 <= max_length cap <= tgt_seq_len");
+    s->m = m; s->N = N; s->rows = rows; s->cap = cap; s->use_cfg = use_cfg;
+    s->status.assign(N, mb200_stream::FREE);
+    s->prompt_len.assign(N, 0); s->max_length.assign(N, 0); s->first_poll.assign(N, 0); s->selections.assign(N, 0); s->done_len.assign(N, 0);
+    MB_CUDA_CHECK(cudaMallocHost(&s->h_rows, (size_t)N * sizeof(RowState)));
+    const int ids_ld = c.tgt_seq_len, Vin = c.vocab_size_in;
+    // vacant rows: finished, one valid token (the frozen selection re-issues the embedding of ids[r][cur_len - 1])
+    std::vector<unsigned char> state(sizeof(GenState) + (size_t)N * sizeof(RowState), 0);
+    GenState* gs = reinterpret_cast<GenState*>(state.data());
+    gs->n_req = N; gs->all_finished = 1;
+    RowState* rs = reinterpret_cast<RowState*>(gs + 1);
+    for (int r = 0; r < N; ++r) { rs[r].cur_len = 1; rs[r].prompt_len = 1; rs[r].max_length = 2; rs[r].finished = 1; }
+    SampleConfig base{};
+    base.B = N; base.use_cfg = use_cfg ? 1 : 0; base.V = c.vocab_size_out; base.ids_ld = ids_ld; base.vflags_ld = Vin; base.temperature = 1.f;
+    std::vector<SampleConfig> cfgs(N, base);
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_state.p, state.data(), state.size(), cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_cfg.p, cfgs.data(), cfgs.size() * sizeof(SampleConfig), cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->g_ids.p, 0, (size_t)N * ids_ld * 8, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->g_vflags.p, 0, (size_t)N * Vin, st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->g_rowslot.p, 0, (size_t)4 * m->max_rows * sizeof(int), st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->g_keyvalid.p, 1, (size_t)m->max_rows * ids_ld, st));       // no pad keys in a stream row
+    MB_CUDA_CHECK(cudaMemsetAsync(m->g_leftpad.p, 0, m->max_rows * sizeof(int), st));
+    MB_CUDA_CHECK(cudaMemsetAsync(m->d_ticket.p, 0, (size_t)m->max_rows * c.heads * sizeof(int), st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));   // the host vectors above are pageable and go out of scope
+    // the step graph; its key never meets a uniform (.., 1) or beam (.., K) graph
+    auto key = std::make_tuple(rows, N, self_splits(cap), -1);
+    auto it = m->graphs.find(key);
+    if (it == m->graphs.end()) {
+        cudaGraph_t graph;
+        if (!m->cap_stream) MB_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
+        MB_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
+        const long long before = g_launch_count;
+        int e1 = token_step(m, rows, N, self_splits(cap), m->cap_stream, m->use_pdl, nullptr, nullptr, true);
+        cudaError_t e = cudaStreamEndCapture(m->cap_stream, &graph);
+        m->graph_nodes[key] = g_launch_count - before;
+        g_launch_count = before;
+        if (e1) return e1;
+        MB_CUDA_CHECK(e);
+        cudaGraphExec_t exec;
+        MB_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
+        cudaGraphDestroy(graph);
+        it = m->graphs.emplace(key, exec).first;
+    }
+    s->step = it->second;
+    s->step_nodes = m->graph_nodes[key];
+    return 0;
+}
+
+// Admits n requests into the lowest free rows (written to rows_out).  Every bound is checked before anything is launched; then the
+// rows' state leaves from the engine's pinned staging buffer and the prompt scan, each request's prefill at its batch-1 shapes, its
+// final-logits GEMV and the list selection of its first token queue behind it, with no host wait.
+int stream_admit(mb200_stream* s, int n, const int32_t* slots, const int64_t* prompt, const int32_t* prompt_off, const int64_t* neg_prompt,
+                 const uint8_t* vflags, const mb200_generate_params* params, int32_t* rows_out, cudaStream_t st) {
+    mb200_model* m = s->m;
+    const auto& c = m->cfg;
+    MB_REQUIRE(slots && prompt && prompt_off && vflags && params && rows_out, "null argument");
+    MB_REQUIRE(prompt_off[0] == 0, "prompt offsets start at 0");
+    MB_REQUIRE((neg_prompt != nullptr) == s->use_cfg, "a negative prompt with every request of a guided stream and with none of an unguided one");
+    std::vector<int> free_rows;
+    for (int r = 0; r < s->N; ++r) if (s->status[r] == mb200_stream::FREE) free_rows.push_back(r);
+    MB_REQUIRE(n >= 1 && n <= (int)free_rows.size(), "the stream has fewer free rows than requests to admit");
+    const int d = c.d_model, V = c.vocab_size_out, ids_ld = c.tgt_seq_len, Vin = c.vocab_size_in, N = s->N, nr = s->use_cfg ? 2 : 1;
+    for (int j = 0; j < n; ++j) {
+        const mb200_generate_params& gp = params[j];
+        const int P = prompt_off[j + 1] - prompt_off[j];
+        MB_REQUIRE(P >= 1 && P < gp.max_length && gp.max_length <= s->cap, "need 1 <= prompt_len < max_length <= the stream's max_length cap for every request");
+        MB_REQUIRE(slots[j] >= 0 && slots[j] < c.max_windows, "encoder slot out of range");
+        MB_REQUIRE((gp.cfg_scale > 1.0f) == s->use_cfg, "classifier-free guidance on every request of a stream or on none");
+        for (int t = prompt_off[j]; t < prompt_off[j + 1]; ++t) {
+            MB_REQUIRE(prompt[t] >= 0 && prompt[t] < Vin, "prompt token id out of range");
+            MB_REQUIRE(!neg_prompt || (neg_prompt[t] >= 0 && neg_prompt[t] < Vin), "negative prompt token id out of range");
+        }
+    }
+    // ---- staging ----
+    MB_CUDA_CHECK(cudaEventSynchronize(m->stage_ev));       // the previous admission's copies left the pinned buffer
+    size_t stage_off = 0;
+    auto stage = [&](size_t n_bytes) -> void* {
+        stage_off = (stage_off + 15) & ~size_t(15);
+        if (stage_off + n_bytes > m->h_stage_bytes) return nullptr;
+        void* h = m->h_stage + stage_off;
+        stage_off += n_bytes;
+        return h;
+    };
+    auto copy = [&](void* dst, const void* h, size_t n_bytes) -> int {
+        MB_CUDA_CHECK(cudaMemcpyAsync(dst, h, n_bytes, cudaMemcpyHostToDevice, st));
+        return 0;
+    };
+    int* list = static_cast<int*>(stage((size_t)n * sizeof(int)));
+    MB_REQUIRE(list, "admission exceeds the staging buffer");
+    std::vector<size_t> pre_off(n);
+    size_t total = 0;
+    for (int j = 0; j < n; ++j) { pre_off[j] = total; total += (size_t)nr * (prompt_off[j + 1] - prompt_off[j]); }
+    long long* pre = static_cast<long long*>(stage(total * 8));
+    MB_REQUIRE(pre, "admission exceeds the staging buffer");
+    // pointers into the pinned buffer for every per-row record; checked all at once before the first copy is issued
+    std::vector<long long*> h_ids(n); std::vector<RowState*> h_rs(n); std::vector<SampleConfig*> h_cfg(n); std::vector<int*> h_slot(n);
+    std::vector<unsigned char*> h_vf(n);
+    for (int j = 0; j < n; ++j) {
+        h_ids[j] = static_cast<long long*>(stage((size_t)ids_ld * 8));
+        h_rs[j] = static_cast<RowState*>(stage(sizeof(RowState)));
+        h_cfg[j] = static_cast<SampleConfig*>(stage(sizeof(SampleConfig)));
+        h_vf[j] = static_cast<unsigned char*>(stage((size_t)Vin));
+        h_slot[j] = static_cast<int*>(stage(4 * sizeof(int)));
+        MB_REQUIRE(h_ids[j] && h_rs[j] && h_cfg[j] && h_vf[j] && h_slot[j], "admission exceeds the staging buffer");
+    }
+    for (int j = 0; j < n; ++j) {
+        const mb200_generate_params& gp = params[j];
+        const int P = prompt_off[j + 1] - prompt_off[j], r = free_rows[j];
+        list[j] = r;
+        for (int i = 0; i < nr; ++i) {      // prefill rows of the request: the negative prompt first (modeling_mapperatorinator.py:243-245)
+            const int64_t* src = (s->use_cfg && i == 0) ? neg_prompt : prompt;
+            for (int t = 0; t < P; ++t) pre[pre_off[j] + (size_t)i * P + t] = src[prompt_off[j] + t];
+        }
+        for (int t = 0; t < ids_ld; ++t) h_ids[j][t] = t < P ? prompt[prompt_off[j] + t] : gp.pad_token_id;
+        *h_rs[j] = RowState{};
+        h_rs[j]->cur_len = P; h_rs[j]->prompt_len = P; h_rs[j]->max_length = gp.max_length; h_rs[j]->min_new_tokens = gp.min_new_tokens;
+        *h_cfg[j] = make_sample_config(&gp, N, s->use_cfg, V, ids_ld);
+        h_cfg[j]->pos_rule_cumsum = 0; h_cfg[j]->vflags_ld = Vin;
+        std::memcpy(h_vf[j], vflags + (size_t)j * Vin, Vin);
+        for (int i = 0; i < 4; ++i) h_slot[j][i] = slots[j];
+    }
+    GenState* gs = m->g_state.as<GenState>();
+    int* rowslot = m->g_rowslot.as<int>();
+    int* d_list = rowslot + 3 * m->max_rows;
+    MB_TRY(copy(d_list, list, (size_t)n * sizeof(int)));
+    MB_TRY(copy(m->g_prefill_ids.p, pre, total * 8));
+    for (int j = 0; j < n; ++j) {
+        const int r = list[j];
+        MB_TRY(copy(m->g_ids.as<long long>() + (size_t)r * ids_ld, h_ids[j], (size_t)ids_ld * 8));
+        MB_TRY(copy(ragged_rows(gs) + r, h_rs[j], sizeof(RowState)));
+        MB_TRY(copy(m->g_cfg.as<SampleConfig>() + r, h_cfg[j], sizeof(SampleConfig)));
+        MB_TRY(copy(m->g_vflags.as<unsigned char>() + (size_t)r * Vin, h_vf[j], (size_t)Vin));
+        for (int i = 0; i < nr; ++i) MB_TRY(copy(rowslot + r + i * N, h_slot[j], sizeof(int)));      // decode rows r, N + r
+        MB_TRY(copy(rowslot + m->max_rows + 2 * r, h_slot[j], 2 * sizeof(int)));                     // the prefill's (slot, slot) pair
+    }
+    MB_CUDA_CHECK(cudaEventRecord(m->stage_ev, st));
+    for (int j = 0; j < n; ++j) {
+        const int r = list[j];
+        s->status[r] = mb200_stream::LIVE;
+        s->prompt_len[r] = prompt_off[j + 1] - prompt_off[j];
+        s->max_length[r] = params[j].max_length;
+        s->first_poll[r] = std::min(std::max(params[j].min_new_tokens, 1), params[j].max_length - s->prompt_len[r]);   // no earlier stop
+        s->selections[r] = 1;
+    }
+    // ---- launches ----
+    MB_TRY(launch_prompt_scan_ragged(m->g_ids.as<long long>(), ids_ld, n, gs, m->g_vflags.as<unsigned char>(), Vin, params[0].time_shift_start,
+                                     params[0].time_shift_end, m->g_lastts.as<int>(), st, d_list));
+    // prefill of request j == the prefill of its batch-1 call, into cache rows r (and N + r); its last-position logits land in the
+    // logits rows of the same index
+    for (int j = 0; j < n; ++j) {
+        const int P = prompt_off[j + 1] - prompt_off[j], r = list[j];
+        MB_TRY(decoder_prefill(m, nr, P, m->g_prefill_ids.as<long long>() + pre_off[j], 0, st, r, N, rowslot + m->max_rows + 2 * r));
+        GemvParams g = final_logits_params(m, nr, m->p_x.as<float>() + (size_t)(P - 1) * d, (long long)P * d);
+        g.seg[0].out += (size_t)r * V; g.seg[0].out_bs = (long long)N * V;
+        MB_TRY(launch_gemv(g, st, false));
+    }
+    // the list selection sets all_finished again if every row of the stream is finished after it
+    MB_CUDA_CHECK(cudaMemsetAsync(&gs->all_finished, 0, sizeof(int), st));
+    MB_TRY(launch_sample_rows(sample_params(m, s->rows), d_list, n, st));
+    for (int j = 0; j < n; ++j) rows_out[j] = list[j];
+    return 0;
+}
+
+// Replays the step graph for one burst (its length to *steps), then reads the rows' state back; the rows that finished are written to
+// done_rows / done_len.
+// The burst is short while requests wait for a row (`waiting` > 0), so a freed row is refilled within a step or two; otherwise it is 16
+// steps, stretched until the first live row could stop and cut at the step where the last one must stop.
+int stream_run(mb200_stream* s, int waiting, int32_t* done_rows, int32_t* done_len, int32_t* n_done, int32_t* steps, cudaStream_t st) {
+    mb200_model* m = s->m;
+    *n_done = 0;
+    *steps = 0;
+    int remaining = 0, earliest = INT32_MAX, live = 0;
+    for (int r = 0; r < s->N; ++r) {
+        if (s->status[r] != mb200_stream::LIVE) continue;
+        ++live;
+        remaining = std::max(remaining, s->max_length[r] - (s->prompt_len[r] + s->selections[r]));
+        earliest = std::min(earliest, s->first_poll[r] - s->selections[r]);
+    }
+    if (!live) return 0;
+    const int burst = std::max(0, std::min(remaining, std::max(waiting > 0 ? 2 : 16, earliest)));
+    for (int i = 0; i < burst; ++i) MB_CUDA_CHECK(cudaGraphLaunch(s->step, st));
+    g_launch_count += (long long)burst * s->step_nodes;
+    *steps = burst;
+    MB_CUDA_CHECK(cudaMemcpyAsync(s->h_rows, ragged_rows(m->g_state.as<GenState>()), (size_t)s->N * sizeof(RowState), cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int r = 0; r < s->N; ++r) {
+        if (s->status[r] != mb200_stream::LIVE) continue;
+        s->selections[r] += burst;
+        const RowState& rs = s->h_rows[r];
+        if (!rs.finished) continue;
+        MB_REQUIRE(rs.cur_len > s->prompt_len[r] && rs.cur_len <= s->max_length[r], "a stream row finished with an out-of-range length");
+        s->status[r] = mb200_stream::DONE;
+        s->done_len[r] = rs.cur_len;
+        done_rows[*n_done] = r; done_len[*n_done] = rs.cur_len; ++*n_done;
+    }
+    return 0;
+}
+
+// Copies a finished row's ids (prompt + generated, done_len of them) into out (host, out_ld wide) and frees the row.  Synchronises `st`.
+int stream_take(mb200_stream* s, int row, int64_t* out, int32_t out_ld, cudaStream_t st) {
+    MB_REQUIRE(row >= 0 && row < s->N && s->status[row] == mb200_stream::DONE, "the row holds no finished request");
+    MB_REQUIRE(out && out_ld >= s->done_len[row], "output row is shorter than the request's ids");
+    MB_CUDA_CHECK(cudaMemcpyAsync(out, s->m->g_ids.as<long long>() + (size_t)row * s->m->cfg.tgt_seq_len, (size_t)s->done_len[row] * 8,
+                                  cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));
+    s->status[row] = mb200_stream::FREE;
+    return 0;
+}
+
+}  // namespace
+
+extern "C" int mb200_stream_open(mb200_model* m, int32_t capacity, int32_t use_cfg, int32_t max_length, mb200_stream** out, void* stream) {
+    MB_REQUIRE(m && m->finalized, "model not finalized");
+    MB_REQUIRE(out, "null argument");
+    MB_REQUIRE(!m->live_stream, "a decode stream is already open on this engine");
+    mb200_stream* s = new mb200_stream();
+    const int e = stream_open(m, s, capacity, use_cfg != 0, max_length, (cudaStream_t)stream);
+    if (e) { stream_release(s); delete s; return e; }
+    m->live_stream = s;
+    *out = s;
+    return 0;
+}
+
+extern "C" int mb200_stream_admit(mb200_stream* s, int32_t n, const int32_t* slots, const int64_t* prompt, const int32_t* prompt_off,
+                                  const int64_t* neg_prompt, const uint8_t* vflags, const mb200_generate_params* params, int32_t* rows_out,
+                                  void* stream) {
+    MB_REQUIRE(s && s->m, "stream not open");
+    return stream_admit(s, n, slots, prompt, prompt_off, neg_prompt, vflags, params, rows_out, (cudaStream_t)stream);
+}
+
+extern "C" int mb200_stream_run(mb200_stream* s, int32_t waiting, int32_t* done_rows, int32_t* done_len, int32_t* n_done, int32_t* steps,
+                                void* stream) {
+    MB_REQUIRE(s && s->m, "stream not open");
+    MB_REQUIRE(done_rows && done_len && n_done && steps, "null argument");
+    return stream_run(s, waiting, done_rows, done_len, n_done, steps, (cudaStream_t)stream);
+}
+
+extern "C" int mb200_stream_take(mb200_stream* s, int32_t row, int64_t* out_ids, int32_t out_ld, void* stream) {
+    MB_REQUIRE(s && s->m, "stream not open");
+    return stream_take(s, row, out_ids, out_ld, (cudaStream_t)stream);
+}
+
+extern "C" void mb200_stream_close(mb200_stream* s) {
+    if (!s) return;
+    if (s->m && s->m->live_stream == s) s->m->live_stream = nullptr;
+    stream_release(s);
+    delete s;
+}
+
 // Ragged batched generate: n_req INDEPENDENT requests in one token loop, each row bit-identical in its ids to its own batch-1
-// mb200_model_generate call.  Prefill runs per request with the shapes of that call (1 row, 2 under classifier-free guidance) straight
-// into the request's cache rows; the first selection and every later token step run all rows together through the ragged per-phase
-// kernels (own length, own split plan, own processor settings, own EOS set per row), one CUDA-graph replay per token.  The two
-// megakernels stay uniform (rows <= 2).  Every bound is checked here, before anything is launched.
+// mb200_model_generate call — a stream of capacity n_req and the largest max_length as its cap, every request admitted at once, run to
+// the end.  Every bound is checked before anything is launched.
 extern "C" int mb200_model_generate_ragged(mb200_model* m, int32_t n_req, const int32_t* slots, const int64_t* prompt, const int32_t* prompt_off,
                                            const int64_t* neg_prompt, const uint8_t* vflags, const mb200_generate_params* params,
                                            int64_t* out_ids, int32_t out_ld, int32_t* out_len, void* stream) {
     MB_REQUIRE(m && m->finalized, "model not finalized");
+    MB_REQUIRE(!m->live_stream, "a decode stream is open on this engine: close it first");
     MB_REQUIRE(slots && prompt && prompt_off && vflags && params && out_ids && out_len, "null argument");
     const auto& c = m->cfg;
     cudaStream_t st = (cudaStream_t)stream;
     const bool use_cfg = neg_prompt != nullptr;
-    const int N = n_req, rows = use_cfg ? 2 * N : N, nr = use_cfg ? 2 : 1;
-    MB_REQUIRE(N >= 1 && rows <= m->max_rows, "requests exceed max_batch (rows double under classifier-free guidance)");
+    const int N = n_req;
+    MB_REQUIRE(N >= 1 && (use_cfg ? 2 * N : N) <= m->max_rows, "requests exceed max_batch (rows double under classifier-free guidance)");
     MB_REQUIRE(prompt_off[0] == 0, "prompt offsets start at 0");
-    const int d = c.d_model, V = c.vocab_size_out, ids_ld = c.tgt_seq_len, Vin = c.vocab_size_in;
-    int n_splits_grid = 1, remaining = 0, first_poll = c.tgt_seq_len;
+    int cap = 2;
     for (int r = 0; r < N; ++r) {
         const mb200_generate_params& gp = params[r];
         const int P = prompt_off[r + 1] - prompt_off[r];
@@ -1106,108 +1392,30 @@ extern "C" int mb200_model_generate_ragged(mb200_model* m, int32_t n_req, const 
         MB_REQUIRE(slots[r] >= 0 && slots[r] < c.max_windows, "encoder slot out of range");
         MB_REQUIRE((gp.cfg_scale > 1.0f) == use_cfg, "classifier-free guidance on every request of a ragged call or on none");
         for (int t = prompt_off[r]; t < prompt_off[r + 1]; ++t) {
-            MB_REQUIRE(prompt[t] >= 0 && prompt[t] < Vin, "prompt token id out of range");
-            MB_REQUIRE(!use_cfg || (neg_prompt[t] >= 0 && neg_prompt[t] < Vin), "negative prompt token id out of range");
+            MB_REQUIRE(prompt[t] >= 0 && prompt[t] < c.vocab_size_in, "prompt token id out of range");
+            MB_REQUIRE(!use_cfg || (neg_prompt[t] >= 0 && neg_prompt[t] < c.vocab_size_in), "negative prompt token id out of range");
         }
-        n_splits_grid = std::max(n_splits_grid, self_splits(gp.max_length));
-        remaining = std::max(remaining, gp.max_length - (P + 1));
-        first_poll = std::min(first_poll, std::min(std::max(gp.min_new_tokens, 1), gp.max_length - P));      // no row can stop earlier
+        cap = std::max(cap, (int)gp.max_length);
     }
-
-    // ---- host-side staging of the call state: one prompt per cache row, no padding anywhere ----
-    const int total = prompt_off[N];
-    std::vector<long long> pre((size_t)nr * total), idsrow((size_t)N * ids_ld, 0);
-    std::vector<size_t> pre_off(N);
-    std::vector<int> rowslot((size_t)3 * m->max_rows, 0);
-    std::vector<unsigned char> state(sizeof(GenState) + (size_t)N * sizeof(RowState), 0);
-    std::vector<SampleConfig> cfgs(N);
-    reinterpret_cast<GenState*>(state.data())->n_req = N;
-    RowState* rs = reinterpret_cast<RowState*>(state.data() + sizeof(GenState));
-    size_t off = 0;
-    for (int r = 0; r < N; ++r) {
-        const mb200_generate_params& gp = params[r];
-        const int P = prompt_off[r + 1] - prompt_off[r];
-        pre_off[r] = off;
-        for (int i = 0; i < nr; ++i) {      // prefill rows of the request: the negative prompt first (modeling_mapperatorinator.py:243-245)
-            const int64_t* src = (use_cfg && i == 0) ? neg_prompt : prompt;
-            for (int t = 0; t < P; ++t) pre[off + (size_t)i * P + t] = src[prompt_off[r] + t];
+    mb200_stream s;
+    int e = stream_open(m, &s, N, use_cfg, cap, st);
+    std::vector<int32_t> rows(N), done_rows(N), done_len(N);
+    if (!e) e = stream_admit(&s, N, slots, prompt, prompt_off, neg_prompt, vflags, params, rows.data(), st);
+    int left = N;
+    while (!e && left > 0) {
+        int32_t n_done = 0, steps = 0;
+        e = stream_run(&s, 0, done_rows.data(), done_len.data(), &n_done, &steps, st);
+        for (int k = 0; !e && k < n_done; ++k) {
+            const int j = done_rows[k];        // all admitted at once into an empty stream: request j holds row j
+            e = stream_take(&s, done_rows[k], out_ids + (size_t)j * out_ld, out_ld, st);
+            out_len[j] = done_len[k];
+            --left;
         }
-        off += (size_t)nr * P;
-        for (int t = 0; t < P; ++t) idsrow[(size_t)r * ids_ld + t] = prompt[prompt_off[r] + t];
-        for (int i = 0; i < nr; ++i) { rowslot[r + i * N] = slots[r]; rowslot[m->max_rows + 2 * r + i] = slots[r]; }
-        rs[r].cur_len = P; rs[r].prompt_len = P; rs[r].max_length = gp.max_length; rs[r].min_new_tokens = gp.min_new_tokens;
-        for (int t = 0; t < ids_ld; ++t) if (t >= P) idsrow[(size_t)r * ids_ld + t] = gp.pad_token_id;
-        cfgs[r] = make_sample_config(&gp, N, use_cfg, V, ids_ld);
-        cfgs[r].pos_rule_cumsum = 0; cfgs[r].vflags_ld = Vin;
     }
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_prefill_ids.p, pre.data(), pre.size() * 8, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_ids.p, idsrow.data(), idsrow.size() * 8, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemsetAsync(m->g_keyvalid.p, 1, (size_t)m->max_rows * ids_ld, st));
-    MB_CUDA_CHECK(cudaMemsetAsync(m->g_leftpad.p, 0, m->max_rows * sizeof(int), st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_rowslot.p, rowslot.data(), rowslot.size() * 4, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_vflags.p, vflags, (size_t)N * Vin, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_state.p, state.data(), state.size(), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_cfg.p, cfgs.data(), cfgs.size() * sizeof(SampleConfig), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemsetAsync(m->d_ticket.p, 0, (size_t)m->max_rows * c.heads * sizeof(int), st));
-    MB_CUDA_CHECK(cudaStreamSynchronize(st));   // host vectors go out of scope; the copies above are from pageable memory
-
-    GenState* gs = m->g_state.as<GenState>();
-    MB_TRY(launch_prompt_scan_ragged(m->g_ids.as<long long>(), ids_ld, N, gs, m->g_vflags.as<unsigned char>(), Vin, cfgs[0].ts_start,
-                                     cfgs[0].ts_end, m->g_lastts.as<int>(), st));
-    // prefill of request r == the prefill of its batch-1 call, into cache rows r (and N + r); its last-position logits land in the
-    // logits rows of the same index, then ONE ragged selection picks every first token
-    for (int r = 0; r < N; ++r) {
-        const int P = prompt_off[r + 1] - prompt_off[r];
-        MB_TRY(decoder_prefill(m, nr, P, m->g_prefill_ids.as<long long>() + pre_off[r], 0, st, r, N, m->g_rowslot.as<int>() + m->max_rows + 2 * r));
-        GemvParams g = final_logits_params(m, nr, m->p_x.as<float>() + (size_t)(P - 1) * d, (long long)P * d);
-        g.seg[0].out += (size_t)r * V; g.seg[0].out_bs = (long long)N * V;
-        MB_TRY(launch_gemv(g, st, false));
-    }
-    MB_TRY(launch_sample(sample_params(m, rows), N, st, false, true));
-
-    // ---- token loop: one replay of the ragged step graph per token; its key never meets a uniform (.., 1) or beam (.., K) graph ----
-    auto key = std::make_tuple(rows, N, n_splits_grid, -1);
-    auto it = m->graphs.find(key);
-    if (it == m->graphs.end()) {
-        cudaGraph_t graph;
-        if (!m->cap_stream) MB_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
-        MB_CUDA_CHECK(cudaStreamSynchronize(st));
-        MB_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
-        const long long before = g_launch_count;
-        int s = token_step(m, rows, N, n_splits_grid, m->cap_stream, m->use_pdl, nullptr, nullptr, true);
-        cudaError_t e = cudaStreamEndCapture(m->cap_stream, &graph);
-        m->graph_nodes[key] = g_launch_count - before;
-        g_launch_count = before;
-        if (s) return s;
-        MB_CUDA_CHECK(e);
-        cudaGraphExec_t exec;
-        MB_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
-        cudaGraphDestroy(graph);
-        it = m->graphs.emplace(key, exec).first;
-    }
-    int produced = 1;
-    while (remaining > 0) {
-        int burst = std::min(remaining, 16);
-        if (first_poll > produced) burst = std::min(remaining, std::max(burst, first_poll - produced));
-        for (int i = 0; i < burst; ++i) MB_CUDA_CHECK(cudaGraphLaunch(it->second, st));
-        g_launch_count += (long long)burst * m->graph_nodes[key];
-        remaining -= burst; produced += burst;
-        MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag, &gs->all_finished, 4, cudaMemcpyDeviceToHost, st));
-        MB_CUDA_CHECK(cudaStreamSynchronize(st));
-        if (*m->h_flag) break;
-    }
-    MB_CUDA_CHECK(cudaMemcpyAsync(state.data(), m->g_state.p, state.size(), cudaMemcpyDeviceToHost, st));
-    MB_CUDA_CHECK(cudaMemcpy2DAsync(out_ids, (size_t)out_ld * 8, m->g_ids.p, (size_t)ids_ld * 8, (size_t)std::min((int)out_ld, ids_ld) * 8, N,
-                                    cudaMemcpyDeviceToHost, st));
-    MB_CUDA_CHECK(cudaStreamSynchronize(st));
-    for (int r = 0; r < N; ++r) {
-        MB_REQUIRE(rs[r].finished && rs[r].cur_len <= params[r].max_length, "ragged token loop ended with an unfinished row");
-        out_len[r] = rs[r].cur_len;
-    }
-    return 0;
+    stream_release(&s);
+    return e;
 }
 
-// beam-search state for max_batch rows, allocated once: captured graphs hold the pointers
 static int ensure_beam_buffers(mb200_model* m) {
     const size_t R = (size_t)m->max_rows, ld = (size_t)m->cfg.tgt_seq_len, V = (size_t)m->cfg.vocab_size_out;
     MB_TRY(m->b_kvsrc.ensure(R * ld * sizeof(int)));
@@ -1245,6 +1453,7 @@ extern "C" int mb200_model_generate_beams(mb200_model* m, const int32_t* slots, 
                                           const mb200_generate_params* gp, int32_t num_beams, int64_t fill_id, int64_t* out_ids,
                                           int32_t* out_len, float* out_scores, void* stream) {
     MB_REQUIRE(m && m->finalized, "model not finalized");
+    MB_REQUIRE(!m->live_stream, "a decode stream is open on this engine: close it first");
     MB_REQUIRE(slots && prompt && vflags && gp && out_ids && out_len && out_scores, "null argument");
     const auto& c = m->cfg;
     cudaStream_t st = (cudaStream_t)stream;
@@ -1382,6 +1591,7 @@ extern "C" int mb200_model_generate_beams(mb200_model* m, const int32_t* slots, 
 static int teacher_forced_hidden(mb200_model* m, const int32_t* slots, int32_t B, const int64_t* ids, const uint8_t* mask, int32_t len,
                                  int32_t position_rule, cudaStream_t st) {
     MB_REQUIRE(m && m->finalized, "model not finalized");
+    MB_REQUIRE(!m->live_stream, "a decode stream is open on this engine: close it first");
     MB_REQUIRE(B >= 1 && B <= m->max_rows && len >= 1 && len <= m->cfg.tgt_seq_len, "bad batch / length");
     const auto& c = m->cfg;
     const int ids_ld = c.tgt_seq_len, d = c.d_model;

@@ -164,22 +164,24 @@ struct GenState {            // device-resident, one per engine
     int ticket;              // last-CTA detection in the sampling kernel
     int all_finished;
     int has_last_scores;
-    int step;                // decode steps since the start of this call (RNG counter)
+    int step;                // decode steps since the start of this call (RNG counter; a ragged row counts its own in RowState)
     int n_req;               // ragged call: un-doubled rows of the call (0 in a uniform call)
     int pad_[6];
 };
 
-// Ragged call (mb200_model_generate_ragged): every request is its own batch-1 call.  The GenState above keeps what the rows share
-// (all rows start together: step, has_last_scores, the tickets); what differs per row follows it IN THE SAME device buffer, so a
+// Ragged call and decode stream (mb200_model_generate_ragged, mb200_stream_*): every request is its own batch-1 call.  The GenState
+// above keeps what the rows share (the tickets, all_finished, n_req); what differs per row follows it IN THE SAME device buffer, so a
 // kernel that holds the GenState pointer finds row b's state at ragged_rows(st)[b].  Decoder row r (2B rows under CFG) belongs to
-// request r % B.
+// request r % B.  Each row counts its own steps, so a request admitted into a running stream draws and looks back as its own call.
 struct RowState {
     int cur_len;             // tokens in this row's ids (prompt + generated); its next token goes to ids[b][cur_len]
     int prompt_len;
     int max_length;
     int min_new_tokens;
-    int finished;            // stopped on its own EOS set or max_length: the row appends nothing more, to its ids or to its cache
-    int pad_[3];
+    int finished;            // stopped on its own EOS set or max_length (or a vacant stream row): appends nothing, to its ids or cache
+    int step;                // selections made since the row's prefill (RNG counter, parity of its look-back scores)
+    int has_last_scores;     // the look-back bias has this row's previous scores
+    int pad_;
 };
 __host__ __device__ inline const RowState* ragged_rows(const GenState* st) { return reinterpret_cast<const RowState*>(st + 1); }
 __host__ __device__ inline RowState* ragged_rows(GenState* st) { return reinterpret_cast<RowState*>(st + 1); }
@@ -285,6 +287,9 @@ struct SampleParams {
 };
 // ragged: cfg / vflags are per-request arrays, st heads a ragged state; row b runs the chain of its own batch-1 call
 int launch_sample(const SampleParams& p, int B, cudaStream_t stream, bool pdl, bool ragged = false);
+// the ragged selection of the n rows in the DEVICE list `rows` only (first token of rows just prefilled into a running stream): one CTA
+// per listed row; no other row's ids, state, embedding or look-back scores are touched
+int launch_sample_rows(const SampleParams& p, const int* rows, int n, cudaStream_t stream);
 
 // ---- beam.cu: beam search (num_beams K <= 4) after the decoder's final logits ---------------------------------------------
 struct BeamParams {
@@ -385,9 +390,10 @@ int mega2_set_poll_sleep(int ns);                 // tuning: nanoseconds to back
 // one-time per call: scan the prompt for the MonotonicTimeShift state (logit_processors.py:149-166)
 int launch_prompt_scan(const long long* ids, long long ids_ld, int B, int P, const unsigned char* vflags, int ts_start, int ts_end,
                        int* last_ts, cudaStream_t stream);
-// the same per request of a ragged call: own prompt length (ragged state `st`) and own flag row
-int launch_prompt_scan_ragged(const long long* ids, long long ids_ld, int B, const GenState* st, const unsigned char* vflags, long long vflags_ld,
-                              int ts_start, int ts_end, int* last_ts, cudaStream_t stream);
+// the same per request of a ragged call: own prompt length (ragged state `st`) and own flag row; rows = DEVICE list of the n rows to
+// scan (null: rows 0 .. n - 1)
+int launch_prompt_scan_ragged(const long long* ids, long long ids_ld, int n, const GenState* st, const unsigned char* vflags, long long vflags_ld,
+                              int ts_start, int ts_end, int* last_ts, cudaStream_t stream, const int* rows = nullptr);
 // prefill embedding: x[b, t] = tok_emb[ids[b, t]] + pos_emb[pos(b, t)]
 int launch_embed(const long long* ids, long long ids_ld, int rows, int B_ids, int P, const int* n_left_pad, int pos_rule_cumsum,
                  const float* tok_emb, const float* pos_emb, int d_model, float* x, cudaStream_t stream);

@@ -207,15 +207,11 @@ class ModelEngine:
         L = out_len.value
         return torch.from_numpy(out.reshape(-1)[: B * L].reshape(B, L).copy())
 
-    def generate_ragged(self, requests: Sequence[tuple], layout: TokenLayout) -> List[torch.Tensor]:
-        """One token loop for independent requests `(slot, prompt ids (P_r,) without padding, generate_kwargs, negative prompt | None)`.
-        Requests may differ in prompt length, `max_length`, `min_new_tokens`, window kind (`lookback_time`, `lookahead_time`,
-        `context_type`), temperatures, `timeshift_bias`, sampling settings and `seed`, `cfg_scale`.  Returns one CPU LongTensor
-        (1, L_r) per request, equal to `generate([slot], prompt[None], None, layout, generate_kwargs, negative_prompt)` of that
-        request alone.  Classifier-free guidance is for every request of the call or for none; beam search has its own call."""
+    def _ragged_args(self, requests: Sequence[tuple], layout: TokenLayout):
+        """Validates independent batch-1 requests `(slot, prompt ids (P_r,) without padding, generate_kwargs, negative prompt | None)` on
+        the host (ValueError before anything is launched) -> (params, vflags, prompt ids back to back, offsets, negative rows | None,
+        slots, guided) in the form of the C ABI's ragged and stream calls."""
         n = len(requests)
-        if n == 0:
-            return []
         params = (_lib.GenerateParamsC * n)()
         vflags = np.zeros((n, layout.vocab_size_in), dtype=np.uint8)
         prompts, negs, cfg_rows = [], [], []
@@ -240,15 +236,27 @@ class ModelEngine:
             prompts.append(ids); negs.append(neg_full)
         if any(cfg_rows) and not all(cfg_rows):
             raise ValueError("classifier-free guidance (negative prompt and cfg_scale > 1) on every request of a ragged call or on none")
-        rows = n * (2 if cfg_rows[0] else 1)
-        if rows > self.max_batch:
-            raise ValueError(f"{n} requests{' x 2 (classifier-free guidance)' if cfg_rows[0] else ''} = {rows} decoder rows; this engine "
-                             f"was built with max_batch={self.max_batch}")
         off = np.zeros(n + 1, dtype=np.int32)
         off[1:] = np.cumsum([len(x) for x in prompts])
         flat = np.ascontiguousarray(np.concatenate(prompts))
         nflat = np.ascontiguousarray(np.concatenate(negs)) if cfg_rows[0] else None
         slots_a = np.ascontiguousarray(np.asarray([int(q[0]) for q in requests], dtype=np.int32))
+        return params, vflags, flat, off, nflat, slots_a, cfg_rows[0]
+
+    def generate_ragged(self, requests: Sequence[tuple], layout: TokenLayout) -> List[torch.Tensor]:
+        """One token loop for independent requests `(slot, prompt ids (P_r,) without padding, generate_kwargs, negative prompt | None)`.
+        Requests may differ in prompt length, `max_length`, `min_new_tokens`, window kind (`lookback_time`, `lookahead_time`,
+        `context_type`), temperatures, `timeshift_bias`, sampling settings and `seed`, `cfg_scale`.  Returns one CPU LongTensor
+        (1, L_r) per request, equal to `generate([slot], prompt[None], None, layout, generate_kwargs, negative_prompt)` of that
+        request alone.  Classifier-free guidance is for every request of the call or for none; beam search has its own call."""
+        n = len(requests)
+        if n == 0:
+            return []
+        params, vflags, flat, off, nflat, slots_a, guided = self._ragged_args(requests, layout)
+        rows = n * (2 if guided else 1)
+        if rows > self.max_batch:
+            raise ValueError(f"{n} requests{' x 2 (classifier-free guidance)' if guided else ''} = {rows} decoder rows; this engine "
+                             f"was built with max_batch={self.max_batch}")
         ld = max(int(params[r].max_length) for r in range(n))
         out = np.zeros((n, ld), dtype=np.int64)
         out_len = np.zeros(n, dtype=np.int32)
@@ -257,6 +265,13 @@ class ModelEngine:
                 self.handle, n, slots_a.ctypes.data, flat.ctypes.data, off.ctypes.data, None if nflat is None else nflat.ctypes.data,
                 vflags.ctypes.data, C.cast(params, C.c_void_p), out.ctypes.data, ld, out_len.ctypes.data, _stream()))
         return [torch.from_numpy(out[r, :out_len[r]].copy())[None] for r in range(n)]
+
+    def open_stream(self, layout: TokenLayout, capacity: int, guidance: bool = False, max_length: Optional[int] = None) -> "DecodeStream":
+        """A decode stream over this engine: a token loop of `capacity` rows into which batch-1 requests are admitted while it runs
+        (continuous batching).  Every request's ids equal its own `generate` call.  `guidance`: every request carries a negative prompt
+        and cfg_scale > 1 (2 decoder rows each), or none does.  `max_length` caps the requests' max_length (default tgt_seq_len).
+        While the stream is open the engine's other token-loop calls refuse; `encode` into slots no live row reads stays allowed."""
+        return DecodeStream(self, layout, capacity, guidance, max_length)
 
     def generate_beams(self, slots: Sequence[int], prompt: torch.Tensor, prompt_mask: Optional[torch.Tensor], layout: TokenLayout,
                        generate_kwargs: dict, negative_prompt: Optional[torch.Tensor] = None,
@@ -409,6 +424,100 @@ class ModelEngine:
         try:
             if getattr(self, "handle", None):
                 self.lib.mb200_model_destroy(self.handle)
+        except Exception:
+            pass
+
+
+class DecodeStream:
+    """An open decode stream of a `ModelEngine` (see `ModelEngine.open_stream`); a context manager that closes it on exit.
+    `admit` puts a request into a free row, `run` advances every live row by a burst of token steps and hands back the requests
+    that finished, whose rows are free again at once."""
+
+    def __init__(self, engine: ModelEngine, layout: TokenLayout, capacity: int, guidance: bool, max_length: Optional[int]):
+        self.engine, self.layout = engine, layout
+        self.capacity, self.guidance = int(capacity), bool(guidance)
+        self.max_length = int(engine.cfg.tgt_seq_len if max_length is None else max_length)
+        rows = self.capacity * (2 if self.guidance else 1)
+        if not 1 <= rows <= engine.max_batch:
+            raise ValueError(f"a stream of {self.capacity} rows{' x 2 (classifier-free guidance)' if self.guidance else ''} = {rows} "
+                             f"decoder rows; this engine was built with max_batch={engine.max_batch}")
+        if not 2 <= self.max_length <= engine.cfg.tgt_seq_len:
+            raise ValueError(f"max_length cap {self.max_length} outside 2..{engine.cfg.tgt_seq_len}")
+        self._busy: Dict[int, int] = {}            # row -> prompt length, from admission until its request is handed back
+        self.steps = 0                             # token steps replayed so far (the first token of a request comes with its admission)
+        self.handle = C.c_void_p()
+        with torch.cuda.device(engine.device):
+            _lib.check(engine.lib.mb200_stream_open(engine.handle, self.capacity, int(self.guidance), self.max_length,
+                                                    C.byref(self.handle), _stream()))
+
+    @property
+    def free_rows(self) -> int:
+        return self.capacity - len(self._busy)
+
+    @property
+    def live_rows(self) -> int:
+        return len(self._busy)
+
+    def admit(self, slot: int, prompt, generate_kwargs: dict, negative_prompt=None) -> int:
+        """Admits one batch-1 request (prompt ids (P,) without padding, its encoder states already in `slot`) into a free row and
+        queues its prefill and first token; returns the row.  Validation and parameters are those of `generate_ragged`."""
+        if not self.handle:
+            raise RuntimeError("the stream is closed")
+        params, vflags, flat, off, nflat, slots_a, guided = self.engine._ragged_args([(slot, prompt, generate_kwargs, negative_prompt)],
+                                                                                     self.layout)
+        if guided != self.guidance:
+            raise ValueError(f"a {'guided' if guided else 'unguided'} request (negative prompt and cfg_scale > 1) does not fit a "
+                             f"{'guided' if self.guidance else 'unguided'} stream")
+        if params[0].max_length > self.max_length:
+            raise ValueError(f"max_length {params[0].max_length} exceeds the stream's cap of {self.max_length}")
+        if not self.free_rows:
+            raise ValueError(f"all {self.capacity} rows of the stream are busy")
+        row = np.zeros(1, dtype=np.int32)
+        with torch.cuda.device(self.engine.device):
+            _lib.check(self.engine.lib.mb200_stream_admit(
+                self.handle, 1, slots_a.ctypes.data, flat.ctypes.data, off.ctypes.data, None if nflat is None else nflat.ctypes.data,
+                vflags.ctypes.data, C.cast(params, C.c_void_p), row.ctypes.data, _stream()))
+        self._busy[int(row[0])] = int(off[1])
+        return int(row[0])
+
+    def run(self, waiting: int = 0) -> List[tuple]:
+        """One burst of token steps over the live rows -> [(row, ids CPU LongTensor (1, L))] for the requests that finished in it
+        (prompt + generated, as `generate` returns them); their rows are free again.  `waiting`: how many requests the caller holds
+        ready to admit — while any wait, bursts are short so that a freed row is refilled within a step or two."""
+        if not self.handle:
+            raise RuntimeError("the stream is closed")
+        done_rows = np.zeros(self.capacity, dtype=np.int32)
+        done_len = np.zeros(self.capacity, dtype=np.int32)
+        n_done, steps = C.c_int32(0), C.c_int32(0)
+        lib = self.engine.lib
+        out = []
+        with torch.cuda.device(self.engine.device):
+            _lib.check(lib.mb200_stream_run(self.handle, int(waiting), done_rows.ctypes.data, done_len.ctypes.data, C.byref(n_done),
+                                            C.byref(steps), _stream()))
+            self.steps += steps.value
+            for k in range(n_done.value):
+                row, L = int(done_rows[k]), int(done_len[k])
+                ids = np.zeros(L, dtype=np.int64)
+                _lib.check(lib.mb200_stream_take(self.handle, row, ids.ctypes.data, L, _stream()))
+                del self._busy[row]
+                out.append((row, torch.from_numpy(ids)[None]))
+        return out
+
+    def close(self) -> None:
+        if getattr(self, "handle", None):
+            self.engine.lib.mb200_stream_close(self.handle)
+            self.handle = C.c_void_p()
+            self._busy.clear()
+
+    def __enter__(self) -> "DecodeStream":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
         except Exception:
             pass
 

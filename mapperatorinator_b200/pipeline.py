@@ -15,6 +15,7 @@ is the terminal gather of the emitted token streams (`gather_token_streams`).
 """
 from __future__ import annotations
 
+from collections import deque
 from typing import Callable, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -116,6 +117,36 @@ class SongDecoder:
                                                 for s, p in zip(live, prompts)], self.layout)
             for s, p, ids in zip(live, prompts, outs):
                 streams[s].append(ids[0, len(p):].tolist())
+        return streams
+
+    def decode_songs_continuous(self, window_counts: Sequence[int], prompt_fn: Callable[[int, int, List[List[int]]], List[int]],
+                                generate_kwargs_fn: Callable[[int, int], dict], windows_per_song: Optional[int] = None
+                                ) -> List[List[List[int]]]:
+        """`decode_songs_ragged` without the per-window barrier: the songs share one decode stream, and song s's window i + 1 is
+        admitted as soon as its window i has finished, whatever the other songs' windows are doing.  Same arguments and slots
+        (song s, window i at slot s * windows_per_song + i); each stream equals `decode_windows` run on that song alone.
+        Returns streams[s][i]."""
+        stride = windows_per_song or max(window_counts, default=0)
+        streams: List[List[List[int]]] = [[] for _ in window_counts]
+        ready = deque(s for s, n in enumerate(window_counts) if n > 0)
+        if not ready:
+            return streams
+        with self.engine.open_stream(self.layout, min(len(ready), self.engine.max_batch)) as stream:
+            live = {}                      # row -> (song, prompt length)
+            while ready or live:
+                while ready and stream.free_rows:
+                    s = ready.popleft()
+                    i = len(streams[s])
+                    p = prompt_fn(s, i, streams[s])
+                    row = stream.admit(s * stride + i, torch.tensor(p, dtype=torch.long), generate_kwargs_fn(s, i))
+                    live[row] = (s, len(p))
+                # a song whose window is running has its next window waiting for that row
+                waiting = len(ready) + sum(1 for s, _ in live.values() if len(streams[s]) + 1 < window_counts[s])
+                for row, ids in stream.run(waiting=waiting):
+                    s, P = live.pop(row)
+                    streams[s].append(ids[0, P:].tolist())
+                    if len(streams[s]) < window_counts[s]:
+                        ready.append(s)
         return streams
 
 

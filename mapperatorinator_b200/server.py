@@ -66,18 +66,7 @@ def model_generate_requests(model, tokenizer, requests):
     n = len(requests)
     if n > model.engine.max_windows:
         raise ValueError(f"{n} requests need {n} encoder slots; this engine was built with max_windows={model.engine.max_windows}")
-    reqs = []
-    for r, (mk, gk) in enumerate(requests):
-        gk = dict(gk)
-        gk.pop("precision", None)
-        ids = mk["decoder_input_ids"]
-        if ids.shape[0] != 1 or mk["inputs"].shape[0] != 1:
-            raise ValueError("every request of a ragged call is a batch-1 call")
-        mask = mk.get("decoder_attention_mask")
-        if isinstance(mask, torch.Tensor) and not bool(mask.all()):
-            raise ValueError("a request of a ragged call carries its prompt without padding")
-        neg = mk.get("negative_prompt")
-        reqs.append((r, ids[0], gk, None if neg is None else neg[0]))
+    reqs = [(r, *_batch1_request(mk, gk)) for r, (mk, gk) in enumerate(requests)]
     start = time.perf_counter()
     model.engine.encode(torch.cat([mk["inputs"] for mk, _ in requests]).to(model.device, torch.float32), slot_begin=0)
     results = model.engine.generate_ragged(reqs, layout)
@@ -87,6 +76,96 @@ def model_generate_requests(model, tokenizer, requests):
         pad_token_id = gk.get("pad_token_id", getattr(tokenizer, "pad_id", None))
         out.append((res, _build_generation_stats(res, mk, pad_token_id, elapsed)))
     return out
+
+
+def _batch1_request(mk: dict, gk: dict):
+    """The rules of a request of a ragged call or stream: batch 1, prompt without padding -> (prompt ids, kwargs, negative prompt)."""
+    gk = dict(gk)
+    gk.pop("precision", None)
+    ids = mk["decoder_input_ids"]
+    if ids.shape[0] != 1 or mk["inputs"].shape[0] != 1:
+        raise ValueError("every request of a ragged call is a batch-1 call")
+    mask = mk.get("decoder_attention_mask")
+    if isinstance(mask, torch.Tensor) and not bool(mask.all()):
+        raise ValueError("a request of a ragged call carries its prompt without padding")
+    neg = mk.get("negative_prompt")
+    return ids[0], gk, None if neg is None else neg[0]
+
+
+@torch.no_grad()
+def model_generate_stream(model, tokenizer, requests, max_rows=None):
+    """Continuous batching: the batch-1 `(model_kwargs, generate_kwargs)` of `requests` (the rules of `model_generate_requests`) go
+    through one decode stream of `max_rows` rows.  `requests` is any iterable, read one request ahead as rows free up; an item `None`
+    means "nothing ready yet" (a server's queue that is momentarily empty) and is skipped without waiting.  Requests are admitted in
+    order as soon as a row is free, each into the encoder slot of its row (the frames of one poll's admissions are encoded as one
+    chunk per run of adjacent slots), and yielded as `(index, ids, stats)` in the order they finish, `index` counting the requests;
+    `(ids, stats)` is what `model_generate` returns for that request, with `elapsed_seconds` from its admission to its hand-back.
+    Every request is guided (negative prompt, cfg_scale > 1) or none is, as the first request is."""
+    layout = TokenLayout.from_tokenizer(tokenizer)
+    engine = model.engine
+    it = iter(requests)
+    end = object()
+    count = 0
+
+    def pull():
+        """(index, model_kwargs, generate_kwargs), None when nothing is ready, `end` when the iterable is exhausted."""
+        nonlocal count
+        item = next(it, end)
+        if item is end or item is None:
+            return item
+        count += 1
+        return (count - 1, *item)
+    pending = pull()
+    while pending is None:
+        pending = pull()
+    if pending is end:
+        return
+    _, first_mk, first_gk = pending
+    guided = first_mk.get("negative_prompt") is not None and float(first_gk.get("cfg_scale", 1.0)) > 1.0
+    per = 2 if guided else 1
+    limit = min(engine.max_windows, engine.max_batch // per)
+    if max_rows is None:
+        max_rows = limit
+    if not 1 <= max_rows <= limit:
+        raise ValueError(f"max_rows={max_rows}: a row needs its own encoder slot and {per} decoder row(s); this engine allows "
+                         f"1..{limit} (max_windows={engine.max_windows}, max_batch={engine.max_batch})")
+    live = {}            # row -> (index, model_kwargs, generate_kwargs, admission time)
+    with engine.open_stream(layout, max_rows, guidance=guided) as stream:
+        while True:
+            free = [r for r in range(max_rows) if r not in live]     # the stream fills its lowest free rows first
+            batch = []
+            while pending is not end:
+                if pending is None:
+                    pending = pull()
+                    if pending is None:
+                        break
+                    continue
+                if len(batch) == len(free):
+                    break                                            # `pending` waits for the next free row
+                idx, mk, gk = pending
+                prompt, gk, neg = _batch1_request(mk, gk)
+                batch.append((free[len(batch)], idx, mk, gk, prompt, neg))
+                pending = None
+            if batch:
+                k = 0
+                while k < len(batch):          # adjacent slots in one encoder chunk
+                    j = k + 1
+                    while j < len(batch) and batch[j][0] == batch[j - 1][0] + 1:
+                        j += 1
+                    engine.encode(torch.cat([b[2]["inputs"] for b in batch[k:j]]).to(model.device, torch.float32), slot_begin=batch[k][0])
+                    k = j
+                for row, idx, mk, gk, prompt, neg in batch:
+                    got = stream.admit(row, prompt, gk, negative_prompt=neg)
+                    assert got == row, (got, row)
+                    live[row] = (idx, mk, gk, time.perf_counter())
+            if not live:
+                if pending is end:
+                    return
+                continue
+            for row, ids in stream.run(waiting=0 if pending is None or pending is end else 1):
+                idx, mk, gk, t0 = live.pop(row)
+                pad_token_id = gk.get("pad_token_id", getattr(tokenizer, "pad_id", None))
+                yield idx, ids, _build_generation_stats(ids, mk, pad_token_id, time.perf_counter() - t0)
 
 
 @torch.no_grad()
