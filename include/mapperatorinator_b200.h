@@ -142,8 +142,9 @@ int mb200_model_generate_ragged(mb200_model* m, int32_t n_req, const int32_t* sl
 /* Decode stream: continuous batching in the token loop.  A ragged token loop with a fixed row capacity: requests are admitted into free
  * rows between token steps and handed back as soon as they finish, and their rows are reused.  Every request's ids are bit-identical to
  * its own batch-1 mb200_model_generate call, whatever step it joins at, whatever the other rows do and whatever its row held before.
- * One stream per engine: while it is open, generate / generate_beams / generate_ragged / forward_logits / score_tokens refuse;
- * mb200_model_encode into slots no live row reads stays allowed.  Beam search does not run in a stream.
+ * One stream per engine: while it is open, generate / generate_beams / generate_ragged / forward_logits / score_tokens, the parity
+ * hooks, mb200_model_profile_step and the option "pdl" refuse; mb200_model_encode into slots no live row reads stays allowed.  Beam
+ * search does not run in a stream.
  *   open:  capacity requests (2 * capacity decoder rows when use_cfg: every request guided, or none), each with max_length <= the
  *          max_length cap.  Captures the stream's token-step graph the first time this shape is seen; synchronises the stream.
  *   admit: n requests, arguments as for mb200_model_generate_ragged (HOST memory), into the lowest free rows (rows_out[n]).  Stages

@@ -42,6 +42,41 @@ struct StepProfiler {
 };
 extern StepProfiler g_prof;
 
+// ---- captured CUDA graphs: a replay counts every node as a launch -------------------------------------------------------
+struct CapturedGraph {
+    cudaGraphExec_t exec = nullptr;
+    long long nodes = 0;          // launches the body counted while it was captured
+    int launch(cudaStream_t st, int times = 1) {
+        for (int i = 0; i < times; ++i) MB_CUDA_CHECK(cudaGraphLaunch(exec, st));
+        g_launch_count += (long long)times * nodes;
+        return 0;
+    }
+};
+
+// Captures `body(stream)` into *out on an engine-owned stream, created on first use (the caller's stream may be the legacy default
+// stream, which cannot capture), once `st` has drained.  The capture launches nothing, so it leaves g_launch_count as it was.
+template <typename Body>
+int capture_graph(cudaStream_t& cap_stream, cudaStream_t st, Body&& body, CapturedGraph* out) {
+    if (!cap_stream) MB_CUDA_CHECK(cudaStreamCreateWithFlags(&cap_stream, cudaStreamNonBlocking));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));
+    cudaGraph_t graph;
+    MB_CUDA_CHECK(cudaStreamBeginCapture(cap_stream, cudaStreamCaptureModeThreadLocal));
+    const long long before = g_launch_count;
+    const int rc = body(cap_stream);
+    const cudaError_t e = cudaStreamEndCapture(cap_stream, &graph);
+    out->nodes = g_launch_count - before;
+    g_launch_count = before;
+    if (rc) {
+        if (e == cudaSuccess) cudaGraphDestroy(graph);
+        return rc;
+    }
+    MB_CUDA_CHECK(e);
+    const cudaError_t ie = cudaGraphInstantiate(&out->exec, graph, 0);
+    cudaGraphDestroy(graph);
+    MB_CUDA_CHECK(ie);
+    return 0;
+}
+
 // ---- activation ids shared by GEMM / GEMV epilogues ------------------------------------------------------------------
 enum Act : int { ACT_NONE = 0, ACT_GELU_ERF = 1, ACT_GELU_TANH = 2, ACT_SILU = 3 };
 

@@ -192,7 +192,7 @@ struct mb200_dit {
     // sampling loop: engine-owned copies of the call's inputs + the step-indexed tables, so the captured step graph never sees a
     // caller pointer
     DevBufD state, z_in, c_in, y_in, noise_in, inpaint_in, dense_in, sched, step_ctr, mods_cur, fmod_cur;
-    std::map<std::tuple<int, int, int, int, int>, std::pair<cudaGraphExec_t, long long>> step_graphs;   // (N, T, mask mode, band, in-paint) -> graph, nodes
+    std::map<std::tuple<int, int, int, int, int>, CapturedGraph> step_graphs;   // (N, T, mask mode, band, in-paint) -> graph
     // sliders of the current chunk (mb200_dit_set_sliders); the step graph is keyed by their presence, the arrays live in fixed buffers
     DevBufD sl_off, sl_idx, sl_end, sl_type, sl_len, sl_pix, sl_err, x0buf;
     int n_sliders = 0, sl_cap = 0, sl_cp_cap = 0;
@@ -217,7 +217,7 @@ extern "C" int mb200_dit_create(mb200_dit** out, const mb200_dit_config* cfg) {
 
 extern "C" void mb200_dit_destroy(mb200_dit* d) {
     if (!d) return;
-    for (auto& g : d->step_graphs) cudaGraphExecDestroy(g.second.first);
+    for (auto& g : d->step_graphs) cudaGraphExecDestroy(g.second.exec);
     if (d->cap_stream) cudaStreamDestroy(d->cap_stream);
     d->gemm.destroy();
     d->attn.destroy();
@@ -528,33 +528,21 @@ extern "C" int mb200_dit_sample_loop(mb200_dit* d, const float* z, const float* 
         // the graph bakes (N, T, mask, in-paint on/off, cfg_scale, steps, the mods / noise table addresses)
         const auto key = std::make_tuple((int)N, (int)T, (int)mk.mask_mode, (int)mk.band + 4096 * d->n_sliders, (inpaint ? 1 : 0) + 2 * steps);
         if (d->graph_cfg_scale != cfg_scale || d->graph_noise != d->noise_in.p || d->graph_mods != d->mods.p) {
-            for (auto& g : d->step_graphs) cudaGraphExecDestroy(g.second.first);
+            for (auto& g : d->step_graphs) cudaGraphExecDestroy(g.second.exec);
             d->step_graphs.clear();
             d->graph_cfg_scale = cfg_scale; d->graph_noise = d->noise_in.p; d->graph_mods = d->mods.p;
         }
         auto it = d->step_graphs.find(key);
         if (it == d->step_graphs.end()) {
-            if (!d->cap_stream) MB_CUDA_CHECK(cudaStreamCreateWithFlags(&d->cap_stream, cudaStreamNonBlocking));
-            cudaGraph_t graph;
-            MB_CUDA_CHECK(cudaStreamBeginCapture(d->cap_stream, cudaStreamCaptureModeThreadLocal));
-            const long long before = g_launch_count;
-            const int s = one_step(d->cap_stream);
-            const cudaError_t e = cudaStreamEndCapture(d->cap_stream, &graph);
-            const long long nodes = g_launch_count - before;
-            g_launch_count = before;
-            if (s) return s;
-            MB_CUDA_CHECK(e);
-            cudaGraphExec_t exec;
-            MB_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
-            cudaGraphDestroy(graph);
+            CapturedGraph g;
+            MB_TRY(capture_graph(d->cap_stream, st, one_step, &g));
             if (d->step_graphs.size() >= 16) {      // bounded cache
-                for (auto& g : d->step_graphs) cudaGraphExecDestroy(g.second.first);
+                for (auto& old : d->step_graphs) cudaGraphExecDestroy(old.second.exec);
                 d->step_graphs.clear();
             }
-            it = d->step_graphs.emplace(key, std::make_pair(exec, nodes)).first;
+            it = d->step_graphs.emplace(key, g).first;
         }
-        for (int k = 0; k < steps; ++k) MB_CUDA_CHECK(cudaGraphLaunch(it->second.first, st));
-        g_launch_count += (long long)steps * it->second.second;
+        MB_TRY(it->second.launch(st, steps));
     }
     MB_CUDA_CHECK(cudaMemcpyAsync(out, d->state.p, state_bytes, cudaMemcpyDeviceToDevice, st));
     if (sl.n > 0) {

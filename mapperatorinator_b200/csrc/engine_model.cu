@@ -6,6 +6,7 @@
 #include <cstring>
 #include <functional>
 #include <map>
+#include <memory>
 #include <tuple>
 #include <unordered_map>
 #include <vector>
@@ -67,18 +68,17 @@ struct mb200_model {
     DevBuf d_attn, d_ticket;            // merged attention heads [rows, d] and the per-(row, head) arrival counters of the split merge
     DevBuf g_state, g_cfg, g_vflags, g_ids, g_prefill_ids, g_keyvalid, g_leftpad, g_rowslot, g_finished, g_lastts, g_lastscores;
     int* h_flag = nullptr;              // pinned
-    unsigned char* h_stage = nullptr;   // pinned staging of a generate call's state (prompt ids, masks, slots, flags, GenState, SampleConfig)
+    unsigned char* h_stage = nullptr;   // pinned staging of a call's state (prompt ids, masks, slots, flags, GenState, SampleConfig, ...)
     size_t h_stage_bytes = 0;
     cudaEvent_t stage_ev = nullptr;     // recorded behind the staging copies: h_stage may be refilled once it has completed
     // graph keys carry B as well as rows: the captured sample kernel's grid is dim3(B), and a CFG call (B = 1, rows = 2) must
     // never replay the graph of a plain batch-2 call (B = 2, rows = 2)
     // ... and the beam count: a beam call ends its token step in the beam kernels and must never replay a greedy graph of equal rows
-    std::map<std::tuple<int, int, int, int>, cudaGraphExec_t> graphs;
-    std::map<std::tuple<int, int, int, int>, long long> graph_nodes;   // (rows, B, n_splits_self, num_beams) -> token-step graph
+    std::map<std::tuple<int, int, int, int>, CapturedGraph> graphs;   // (rows, B, n_splits_self, num_beams) -> token-step graph
     bool use_pdl = false;
     cudaStream_t cap_stream = nullptr;
     std::map<std::tuple<int, int, int, int>, int> prefill_seen;                                   // (rows, B, P, position rule)
-    std::map<std::tuple<int, int, int, int>, std::pair<cudaGraphExec_t, long long>> prefill_graphs;   // -> graph + node count
+    std::map<std::tuple<int, int, int, int>, CapturedGraph> prefill_graphs;
     // persistent megakernel path
     int enc_graph = 1;                  // replay single-window encodes as a CUDA graph (option "enc_graph")
     int trace_cta = 0;                  // CTA whose phases the dataflow megakernel's TRACE instantiation stamps
@@ -86,16 +86,16 @@ struct mb200_model {
     DevBuf ll_arena;                    // exchange buffers of the dataflow megakernel (rows <= 2)
     MegaLL ll{};
     size_t ll_bytes = 0;
-    std::map<std::tuple<int, int, int>, std::pair<DevBuf*, int>> mega2_phases;   // (rows, B, n_splits_self) -> device phase table
+    // (driver, rows, B, n_splits_self) -> the megakernel's device phase table and its length
+    std::map<std::tuple<int, int, int, int>, std::pair<std::unique_ptr<DevBuf>, int>> phase_tables;
     int num_sms = 0;                    // 0 = no cooperative launch -> no megakernel
     int num_sms_phys = 0;
     DevBuf g_megasync;                  // [0] grid-barrier counter, [8] error flag
     DevBuf mega_trace;                  // optional per-phase clock64 stamps (option "mega_trace")
     cudaEvent_t mega_ev[2] = {nullptr, nullptr};
     double mega_ms = 0.0; long long mega_launches = 0, mega_tokens = 0;   // CUDA-event time of every megakernel launch
-    std::map<std::pair<int, int>, std::pair<DevBuf*, int>> mega_phases;   // (rows, n_splits_self) -> device phase table
     DevBuf w_pcm;                       // single-window encode: engine-owned copy of the window's PCM (the captured graph reads it)
-    std::map<int, std::pair<cudaGraphExec_t, long long>> enc_graphs;   // slot -> captured single-window encode (the drop-in per-call pattern), node count
+    std::map<int, CapturedGraph> enc_graphs;   // slot -> captured single-window encode (the drop-in per-call pattern)
     std::map<int, int> enc_seen;
     // beam search state (allocated at the first beam call for max_batch rows, then fixed: captured graphs hold the pointers)
     DevBuf b_kvsrc, b_logprobs, b_cand, b_runscore, b_finids[2], b_finscore, b_finlen, b_finflag, b_unsat;
@@ -159,6 +159,80 @@ int layernorm(const float* x, float* y, const float* w, const float* b, int rows
     return launch_layernorm(p, st);
 }
 
+// Every call that writes the token loop's state (ids, GenState, SampleConfig, flag rows, logits rows, token-step graphs) refuses while a
+// decode stream owns that state.
+int token_loop_free(const mb200_model* m) {
+    MB_REQUIRE(!m->live_stream, "a decode stream is open on this engine: close it first");
+    return 0;
+}
+
+// A call's host state leaves from the engine's pinned staging buffer, so its copies are asynchronous and the launches behind them
+// queue with no host wait.  One use: begin() waits until the previous use's copies have left the buffer; reserve() every record and
+// check fits(), so that the capacity is checked before the first copy; fill the records; upload() each; end() records the event
+// begin() waits for.
+struct Stager {
+    mb200_model* m;
+    cudaStream_t st;
+    size_t off = 0;
+    int begin() {
+        MB_CUDA_CHECK(cudaEventSynchronize(m->stage_ev));
+        off = 0;
+        return 0;
+    }
+    template <typename T> T* reserve(size_t n) {      // n elements, 16-byte aligned; past the capacity only fits() may be called
+        off = (off + 15) & ~size_t(15);
+        T* rec = reinterpret_cast<T*>(m->h_stage + off);
+        off += n * sizeof(T);
+        return rec;
+    }
+    int fits() const {
+        MB_REQUIRE(off <= m->h_stage_bytes, "call state exceeds the staging buffer");
+        return 0;
+    }
+    template <typename T> int upload(void* dst, const T* rec, size_t n) {
+        MB_CUDA_CHECK(cudaMemcpyAsync(dst, rec, n * sizeof(T), cudaMemcpyHostToDevice, st));
+        return 0;
+    }
+    int end() {
+        MB_CUDA_CHECK(cudaEventRecord(m->stage_ev, st));
+        return 0;
+    }
+};
+
+// The prefill rows of a prompt call.  Row r holds item item_of(r) of `prompt` (of `neg_prompt` for the first n_neg rows, masked by
+// `neg_mask` when given, else by `mask`): its P ids in pre [rows, P], its key mask in keyvalid [rows, tgt_seq_len] (1 from P on), the
+// count of its leading masked keys in leftpad [rows] and its item's encoder slot in rowslot [rows].  Every slot and every token id is
+// checked before any record is written.
+template <typename ItemOf>
+int build_prompt_rows(const mb200_model* m, int rows, int P, ItemOf item_of, int n_neg, const int32_t* slots, const int64_t* prompt,
+                      const uint8_t* mask, const int64_t* neg_prompt, const uint8_t* neg_mask, long long* pre, unsigned char* keyvalid,
+                      int* leftpad, int* rowslot) {
+    const auto& c = m->cfg;
+    const int ids_ld = c.tgt_seq_len;
+    for (int r = 0; r < rows; ++r) {
+        const int b = item_of(r);
+        const int64_t* src = (r < n_neg ? neg_prompt : prompt) + (size_t)b * P;
+        MB_REQUIRE(slots[b] >= 0 && slots[b] < c.max_windows, "encoder slot out of range");
+        for (int t = 0; t < P; ++t) MB_REQUIRE(src[t] >= 0 && src[t] < c.vocab_size_in, "token id out of range");
+    }
+    for (int r = 0; r < rows; ++r) {
+        const int b = item_of(r);
+        const int64_t* src = (r < n_neg ? neg_prompt : prompt) + (size_t)b * P;
+        const uint8_t* msk = r < n_neg && neg_mask ? neg_mask : mask;
+        unsigned char* kv = keyvalid + (size_t)r * ids_ld;
+        std::memset(kv, 1, ids_ld);
+        int npad = 0; bool seen = false;
+        for (int t = 0; t < P; ++t) {
+            pre[(size_t)r * P + t] = src[t];
+            kv[t] = msk ? (msk[(size_t)b * P + t] != 0) : 1;
+            if (!kv[t] && !seen) ++npad; else seen = true;
+        }
+        leftpad[r] = npad;
+        rowslot[r] = slots[b];
+    }
+    return 0;
+}
+
 }  // namespace
 
 // =====================================================================================================================
@@ -188,13 +262,11 @@ extern "C" int mb200_model_create(mb200_model** out, const mb200_model_config* c
 
 extern "C" void mb200_model_destroy(mb200_model* m) {
     if (!m) return;
-    for (auto& g : m->graphs) cudaGraphExecDestroy(g.second);
-    for (auto& g : m->prefill_graphs) cudaGraphExecDestroy(g.second.first);
-    for (auto& g : m->enc_graphs) cudaGraphExecDestroy(g.second.first);
+    for (auto& g : m->graphs) cudaGraphExecDestroy(g.second.exec);
+    for (auto& g : m->prefill_graphs) cudaGraphExecDestroy(g.second.exec);
+    for (auto& g : m->enc_graphs) cudaGraphExecDestroy(g.second.exec);
     m->gemm.destroy();
     m->attn.destroy();
-    for (auto& kv : m->mega_phases) delete kv.second.first;
-    for (auto& kv : m->mega2_phases) delete kv.second.first;
     for (auto& e : m->mega_ev) if (e) cudaEventDestroy(e);
     if (m->cap_stream) cudaStreamDestroy(m->cap_stream);
     mel_plan_destroy(m->mel);
@@ -351,6 +423,8 @@ extern "C" int mb200_model_finalize(mb200_model* m) {
         m->h_stage_bytes = tgt * 8 * 2 + tgt + (size_t)2 * m->max_rows * 4 + c.vocab_size_in + sizeof(GenState) + sizeof(SampleConfig) + 8 * 16;
         // a stream admission of up to max_rows requests: per row a flag row, RowState, SampleConfig, slot entries and their alignment
         m->h_stage_bytes += (size_t)m->max_rows * (c.vocab_size_in + sizeof(RowState) + sizeof(SampleConfig) + 16 + 5 * 16) + 16;
+        // a beam call: its source-row table, the running and finished scores, and their alignment
+        m->h_stage_bytes += tgt * 4 + (size_t)2 * m->max_rows * 4 + 3 * 16;
         MB_CUDA_CHECK(cudaMallocHost(&m->h_stage, m->h_stage_bytes));
         MB_CUDA_CHECK(cudaEventCreateWithFlags(&m->stage_ev, cudaEventDisableTiming));
     }
@@ -484,7 +558,7 @@ extern "C" int mb200_model_encode(mb200_model* m, const float* pcm, int32_t n_wi
         MB_TRY(m->w_attn.ensure((size_t)chunk * T * d * 4));
         MB_TRY(m->w_ffn.ensure((size_t)chunk * T * c.ffn_dim * 4));
         m->enc_chunk = chunk;
-        for (auto& g : m->enc_graphs) cudaGraphExecDestroy(g.second.first);      // the captured encodes point into the old workspaces
+        for (auto& g : m->enc_graphs) cudaGraphExecDestroy(g.second.exec);      // the captured encodes point into the old workspaces
         m->enc_graphs.clear(); m->enc_seen.clear();
     }
     const long long n_samples = (long long)(c.src_seq_len - 1) * c.mel.hop_length;
@@ -499,26 +573,13 @@ extern "C" int mb200_model_encode(mb200_model* m, const float* pcm, int32_t n_wi
         MB_TRY(m->w_pcm.ensure((size_t)n_samples * sizeof(float)));
         auto git = m->enc_graphs.find(slot_begin);
         if (git == m->enc_graphs.end()) {
-            if (!m->cap_stream) MB_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
-            MB_CUDA_CHECK(cudaStreamSynchronize(st));
-            cudaGraph_t graph;
-            MB_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
-            const long long before = g_launch_count;
-            int rc = encode_chunk(m, m->w_pcm.as<float>(), 1, slot_begin, nullptr, m->cap_stream);
-            cudaError_t e = cudaStreamEndCapture(m->cap_stream, &graph);
-            const long long nodes = g_launch_count - before;
-            g_launch_count = before;
-            if (rc) return rc;
-            MB_CUDA_CHECK(e);
-            cudaGraphExec_t exec;
-            MB_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
-            cudaGraphDestroy(graph);
-            git = m->enc_graphs.emplace(slot_begin, std::make_pair(exec, nodes)).first;
+            CapturedGraph g;
+            MB_TRY(capture_graph(m->cap_stream, st, [&](cudaStream_t cs) { return encode_chunk(m, m->w_pcm.as<float>(), 1, slot_begin, nullptr, cs); },
+                                 &g));
+            git = m->enc_graphs.emplace(slot_begin, g).first;
         }
         MB_CUDA_CHECK(cudaMemcpyAsync(m->w_pcm.p, pcm, (size_t)n_samples * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        MB_CUDA_CHECK(cudaGraphLaunch(git->second.first, st));
-        g_launch_count += git->second.second;
-        return 0;
+        return git->second.launch(st);
     }
     for (int i = 0; i < n_windows; i += m->enc_chunk) {
         int n = std::min(m->enc_chunk, n_windows - i);
@@ -741,42 +802,68 @@ static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaSt
     return 0;
 }
 
-// The persistent path: all remaining tokens of the call in one cooperative launch (rows <= 2, weight slices must fit).
-// `before_sync` enqueues the caller's read-backs ahead of the launch's closing sync, so the call needs only that one host wait.
-static int run_megakernel(mb200_model* m, int rows, int B, int n_splits_self, int max_steps, cudaStream_t st,
-                          const std::function<int()>& before_sync) {
-    auto key = std::make_pair(rows, n_splits_self);
-    auto it = m->mega_phases.find(key);
-    if (it == m->mega_phases.end()) {
+// The device copy of a megakernel's phase table for (rows, B, n_splits_self): token_step's phase list, annotated by `annotate` for the
+// kernel that reads it, built the first time the key is met.
+template <typename Phase, typename Annotate>
+static int phase_table(mb200_model* m, int driver, int rows, int B, int n_splits_self, cudaStream_t st, Annotate annotate,
+                       const Phase** table, int* n_phases) {
+    const auto key = std::make_tuple(driver, rows, B, n_splits_self);
+    auto it = m->phase_tables.find(key);
+    if (it == m->phase_tables.end()) {
         std::vector<MegaPhase> phases;
         MB_TRY(token_step(m, rows, B, n_splits_self, st, false, &phases));
-        DevBuf* buf = new DevBuf();
-        MB_TRY(buf->ensure(phases.size() * sizeof(MegaPhase)));
-        MB_CUDA_CHECK(cudaMemcpy(buf->p, phases.data(), phases.size() * sizeof(MegaPhase), cudaMemcpyHostToDevice));
-        it = m->mega_phases.emplace(key, std::make_pair(buf, (int)phases.size())).first;
+        std::vector<Phase> annotated(phases.size());
+        MB_TRY(annotate(phases, annotated));
+        std::unique_ptr<DevBuf> buf(new DevBuf());
+        MB_TRY(buf->ensure(annotated.size() * sizeof(Phase)));
+        MB_CUDA_CHECK(cudaMemcpy(buf->p, annotated.data(), annotated.size() * sizeof(Phase), cudaMemcpyHostToDevice));
+        it = m->phase_tables.emplace(key, std::make_pair(std::move(buf), (int)annotated.size())).first;
     }
+    *table = it->second.first->template as<Phase>();
+    *n_phases = it->second.second;
+    return 0;
+}
+
+// One persistent launch of the token loop: clears the grid-sync words (g_megasync[0] the barrier counter, [8] the error flag, [9..11]
+// where a timed-out wait was), times `launch` with CUDA events, reads cur_len before and after it into h_flag[2] / h_flag[3] and the
+// error words into h_flag[1] / h_flag[4..6].  `before_sync` enqueues the caller's read-backs ahead of the closing sync, so the call
+// needs only that one host wait.  The error flag is the caller's to interpret.
+static int mega_launch(mb200_model* m, cudaStream_t st, const std::function<int()>& launch, const std::function<int()>& before_sync) {
     MB_TRY(m->g_megasync.ensure(64));
     MB_CUDA_CHECK(cudaMemsetAsync(m->g_megasync.p, 0, 64, st));
-    MegaParams mp{};
-    mp.phases = it->second.first->as<MegaPhase>(); mp.n_phases = it->second.second; mp.first_gemv = 0;
-    mp.sample = sample_params(m, rows); mp.st = m->g_state.as<GenState>();
-    mp.sync_counter = m->g_megasync.as<unsigned int>(); mp.error_flag = m->g_megasync.as<int>() + 8;
-    mp.max_steps = max_steps; mp.row_slot = m->g_rowslot.as<int>();
-    mp.trace = m->mega_trace.p ? m->mega_trace.as<unsigned long long>() : nullptr; mp.trace_step = 8;
     if (!m->mega_ev[0]) { MB_CUDA_CHECK(cudaEventCreate(&m->mega_ev[0])); MB_CUDA_CHECK(cudaEventCreate(&m->mega_ev[1])); }
     MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 2, &m->g_state.as<GenState>()->cur_len, 4, cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaEventRecord(m->mega_ev[0], st));
-    MB_TRY(launch_megakernel(mp, m->num_sms, st));
+    MB_TRY(launch());
     MB_CUDA_CHECK(cudaEventRecord(m->mega_ev[1], st));
     MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 1, m->g_megasync.as<int>() + 8, 4, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 4, m->g_megasync.as<int>() + 9, 12, cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 3, &m->g_state.as<GenState>()->cur_len, 4, cudaMemcpyDeviceToHost, st));
     MB_TRY(before_sync());
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
-    {
-        float ms = 0.f;
-        MB_CUDA_CHECK(cudaEventElapsedTime(&ms, m->mega_ev[0], m->mega_ev[1]));
-        m->mega_ms += ms; m->mega_launches += 1; m->mega_tokens += m->h_flag[3] - m->h_flag[2];
-    }
+    float ms = 0.f;
+    MB_CUDA_CHECK(cudaEventElapsedTime(&ms, m->mega_ev[0], m->mega_ev[1]));
+    m->mega_ms += ms; m->mega_launches += 1; m->mega_tokens += m->h_flag[3] - m->h_flag[2];
+    return 0;
+}
+
+// The persistent path: all remaining tokens of the call in one cooperative launch (rows <= 2, weight slices must fit).
+static int run_megakernel(mb200_model* m, int rows, int B, int n_splits_self, int max_steps, cudaStream_t st,
+                          const std::function<int()>& before_sync) {
+    const MegaPhase* table = nullptr;
+    int n_phases = 0;
+    auto as_is = [](const std::vector<MegaPhase>& phases, std::vector<MegaPhase>& p1) { p1 = phases; return 0; };
+    MB_TRY(phase_table(m, 1, rows, B, n_splits_self, st, as_is, &table, &n_phases));
+    auto launch = [&]() -> int {
+        MegaParams mp{};
+        mp.phases = table; mp.n_phases = n_phases; mp.first_gemv = 0;
+        mp.sample = sample_params(m, rows); mp.st = m->g_state.as<GenState>();
+        mp.sync_counter = m->g_megasync.as<unsigned int>(); mp.error_flag = m->g_megasync.as<int>() + 8;
+        mp.max_steps = max_steps; mp.row_slot = m->g_rowslot.as<int>();
+        mp.trace = m->mega_trace.p ? m->mega_trace.as<unsigned long long>() : nullptr; mp.trace_step = 8;
+        return launch_megakernel(mp, m->num_sms, st);
+    };
+    MB_TRY(mega_launch(m, st, launch, before_sync));
     MB_REQUIRE(m->h_flag[1] == 0, m->h_flag[1] == 1 ? "megakernel grid barrier timed out" : "megakernel weight copy timed out");
     return 0;
 }
@@ -784,12 +871,7 @@ static int run_megakernel(mb200_model* m, int rows, int B, int n_splits_self, in
 // The dataflow path: same phase list, each phase annotated with the exchange buffers it reads / writes.
 static int run_megakernel2(mb200_model* m, int rows, int B, int n_splits_self, int max_steps, cudaStream_t st,
                            const std::function<int()>& before_sync) {
-    auto key = std::make_tuple(rows, B, n_splits_self);
-    auto it = m->mega2_phases.find(key);
-    if (it == m->mega2_phases.end()) {
-        std::vector<MegaPhase> phases;
-        MB_TRY(token_step(m, rows, B, n_splits_self, st, false, &phases));
-        std::vector<Mega2Phase> p2(phases.size());
+    auto annotate = [&](const std::vector<MegaPhase>& phases, std::vector<Mega2Phase>& p2) -> int {
         const float *dx = m->d_x.as<float>(), *dq = m->d_q.as<float>(), *dh = m->d_h.as<float>(), *datt = m->d_attn.as<float>(),
                     *dlog = m->d_logits.as<float>();
         for (size_t i = 0; i < phases.size(); ++i) {
@@ -824,43 +906,30 @@ static int run_megakernel2(mb200_model* m, int rows, int B, int n_splits_self, i
                 q.n_active = (g.N + rpc - 1) / rpc;
             }
         }
-        DevBuf* buf = new DevBuf();
-        MB_TRY(buf->ensure(p2.size() * sizeof(Mega2Phase)));
-        MB_CUDA_CHECK(cudaMemcpy(buf->p, p2.data(), p2.size() * sizeof(Mega2Phase), cudaMemcpyHostToDevice));
-        it = m->mega2_phases.emplace(key, std::make_pair(buf, (int)p2.size())).first;
-    }
-    MB_TRY(m->g_megasync.ensure(64));
-    MB_CUDA_CHECK(cudaMemsetAsync(m->g_megasync.p, 0, 64, st));
+        return 0;
+    };
+    const Mega2Phase* table = nullptr;
+    int n_phases = 0;
+    MB_TRY(phase_table(m, 2, rows, B, n_splits_self, st, annotate, &table, &n_phases));
     MB_CUDA_CHECK(cudaMemsetAsync(m->ll_arena.p, 0, m->ll_bytes, st));        // tag 0 = "nothing here yet"
-    Mega2Params mp{};
-    mp.phases = it->second.first->as<Mega2Phase>(); mp.n_phases = it->second.second;
-    mp.sample = sample_params(m, rows); mp.st = m->g_state.as<GenState>();
-    mp.ll = m->ll; mp.error_flag = m->g_megasync.as<int>() + 8;
-    mp.sample.ll_logits = m->ll.logits; mp.sample.ll_x_out = m->ll.x; mp.sample.ll_hdr = m->ll.hdr; mp.sample.ll_err = mp.error_flag;
-    mp.sample.ll_reps = m->ll.reps; mp.sample.ll_x_rep = m->ll.x_rep;
-    mp.max_steps = max_steps; mp.row_slot = m->g_rowslot.as<int>(); mp.x_in = m->d_x.as<float>();
-    mp.rows = rows; mp.d_model = m->cfg.d_model; mp.V = m->cfg.vocab_size_out; mp.ffn_dim = m->cfg.ffn_dim; mp.trace_cta = m->trace_cta;
-    mp.trace = m->mega_trace.p ? m->mega_trace.as<unsigned long long>() : nullptr; mp.trace_step = 8;
-    if (!m->mega_ev[0]) { MB_CUDA_CHECK(cudaEventCreate(&m->mega_ev[0])); MB_CUDA_CHECK(cudaEventCreate(&m->mega_ev[1])); }
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 2, &m->g_state.as<GenState>()->cur_len, 4, cudaMemcpyDeviceToHost, st));
-    MB_CUDA_CHECK(cudaEventRecord(m->mega_ev[0], st));
-    MB_TRY(launch_megakernel2(mp, m->num_sms, st));
-    MB_CUDA_CHECK(cudaEventRecord(m->mega_ev[1], st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 1, m->g_megasync.as<int>() + 8, 4, cudaMemcpyDeviceToHost, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 4, m->g_megasync.as<int>() + 9, 12, cudaMemcpyDeviceToHost, st));   // where a timed-out wait was
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 3, &m->g_state.as<GenState>()->cur_len, 4, cudaMemcpyDeviceToHost, st));
-    MB_TRY(before_sync());
-    MB_CUDA_CHECK(cudaStreamSynchronize(st));
-    {
-        float ms = 0.f;
-        MB_CUDA_CHECK(cudaEventElapsedTime(&ms, m->mega_ev[0], m->mega_ev[1]));
-        m->mega_ms += ms; m->mega_launches += 1; m->mega_tokens += m->h_flag[3] - m->h_flag[2];
-    }
+    auto launch = [&]() -> int {
+        Mega2Params mp{};
+        mp.phases = table; mp.n_phases = n_phases;
+        mp.sample = sample_params(m, rows); mp.st = m->g_state.as<GenState>();
+        mp.ll = m->ll; mp.error_flag = m->g_megasync.as<int>() + 8;
+        mp.sample.ll_logits = m->ll.logits; mp.sample.ll_x_out = m->ll.x; mp.sample.ll_hdr = m->ll.hdr; mp.sample.ll_err = mp.error_flag;
+        mp.sample.ll_reps = m->ll.reps; mp.sample.ll_x_rep = m->ll.x_rep;
+        mp.max_steps = max_steps; mp.row_slot = m->g_rowslot.as<int>(); mp.x_in = m->d_x.as<float>();
+        mp.rows = rows; mp.d_model = m->cfg.d_model; mp.V = m->cfg.vocab_size_out; mp.ffn_dim = m->cfg.ffn_dim; mp.trace_cta = m->trace_cta;
+        mp.trace = m->mega_trace.p ? m->mega_trace.as<unsigned long long>() : nullptr; mp.trace_step = 8;
+        return launch_megakernel2(mp, m->num_sms, st);
+    };
+    MB_TRY(mega_launch(m, st, launch, before_sync));
     if (m->h_flag[1] == 4) {
         const unsigned tag = (unsigned)m->h_flag[6];
         MB_REQUIRE(false, "dataflow megakernel: a wait for tagged data timed out (CTA " + std::to_string(m->h_flag[4]) + ", thread " +
                               std::to_string(m->h_flag[5]) + ", expected tag " + std::to_string(tag) + " = step " + std::to_string((int)(tag / 128) - 1) +
-                              " phase " + std::to_string((int)(tag % 128) - 1) + " of " + std::to_string(mp.n_phases) + ", splits " +
+                              " phase " + std::to_string((int)(tag % 128) - 1) + " of " + std::to_string(n_phases) + ", splits " +
                               std::to_string(n_splits_self) + ", rows " + std::to_string(rows) + ")");
     }
     MB_REQUIRE(m->h_flag[1] == 0, m->h_flag[1] == 2 ? "dataflow megakernel: weight copy timed out" : "dataflow megakernel: a wait for tagged data timed out");
@@ -892,12 +961,26 @@ static SampleConfig make_sample_config(const mb200_generate_params* gp, int B, b
     return sc;
 }
 
+// Replays a token-step graph in bursts of 16 steps, the first one at least first_burst_min long, polling all_finished after each,
+// until every row finished or `remaining` steps ran.
+static int replay_until_finished(mb200_model* m, CapturedGraph& graph, int remaining, int first_burst_min, cudaStream_t st) {
+    for (int burst_min = first_burst_min; remaining > 0; burst_min = 0) {
+        const int burst = std::min(remaining, std::max(16, burst_min));
+        MB_TRY(graph.launch(st, burst));
+        remaining -= burst;
+        MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag, &m->g_state.as<GenState>()->all_finished, 4, cudaMemcpyDeviceToHost, st));
+        MB_CUDA_CHECK(cudaStreamSynchronize(st));
+        if (*m->h_flag) break;
+    }
+    return 0;
+}
+
 // =====================================================================================================================
 extern "C" int mb200_model_generate(mb200_model* m, const int32_t* slots, int32_t B, const int64_t* prompt, const uint8_t* prompt_mask,
                                     int32_t P, const int64_t* neg_prompt, const uint8_t* neg_mask, const uint8_t* vflags,
                                     const mb200_generate_params* gp, int64_t* out_ids, int32_t* out_len, void* stream) {
     MB_REQUIRE(m && m->finalized, "model not finalized");
-    MB_REQUIRE(!m->live_stream, "a decode stream is open on this engine: close it first");
+    MB_TRY(token_loop_free(m));
     MB_REQUIRE(slots && prompt && vflags && gp && out_ids && out_len, "null argument");
     const auto& c = m->cfg;
     cudaStream_t st = (cudaStream_t)stream;
@@ -905,68 +988,43 @@ extern "C" int mb200_model_generate(mb200_model* m, const int32_t* slots, int32_
     const int rows = use_cfg ? 2 * B : B;
     MB_REQUIRE(B >= 1 && rows <= m->max_rows, "batch exceeds max_batch (rows double under classifier-free guidance)");
     MB_REQUIRE(P >= 1 && P < gp->max_length && gp->max_length <= c.tgt_seq_len, "need 1 <= prompt_len < max_length <= tgt_seq_len");
-    for (int b = 0; b < B; ++b) MB_REQUIRE(slots[b] >= 0 && slots[b] < c.max_windows, "encoder slot out of range");
-    const int d = c.d_model, H = c.heads, T = c.src_seq_len / 2, V = c.vocab_size_out;
+    const int d = c.d_model, V = c.vocab_size_out;
     const int ids_ld = c.tgt_seq_len;
 
-    // ---- host-side staging of the call state ----
-    std::vector<long long> pre((size_t)rows * P), idsrow((size_t)B * ids_ld, (long long)gp->pad_token_id);
-    std::vector<unsigned char> kv((size_t)rows * ids_ld, 1);
-    std::vector<int> leftpad(rows, 0), rowslot(rows);
-    for (int r = 0; r < rows; ++r) {
-        const int b = r % B;
-        const bool neg_row = use_cfg && r < B;   // first half carries the negative prompt (modeling_mapperatorinator.py:243-245)
-        const int64_t* src = neg_row ? neg_prompt : prompt;
-        const uint8_t* msk = neg_row ? (neg_mask ? neg_mask : prompt_mask) : prompt_mask;
-        int npad = 0; bool seen = false;
-        for (int t = 0; t < P; ++t) {
-            long long tok = src[(size_t)b * P + t];
-            MB_REQUIRE(tok >= 0 && tok < c.vocab_size_in, "prompt token id out of range");
-            pre[(size_t)r * P + t] = tok;
-            unsigned char ok = msk ? (msk[(size_t)b * P + t] != 0) : 1;
-            kv[(size_t)r * ids_ld + t] = ok;
-            if (!ok && !seen) ++npad; else seen = true;
-        }
-        leftpad[r] = npad;
-        rowslot[r] = slots[b];
-    }
+    // ---- call state: row r is item r % B; under CFG rows [0, B) carry the negative prompt (modeling_mapperatorinator.py:243-245) ----
+    Stager sg{m, st};
+    MB_TRY(sg.begin());
+    long long* pre = sg.reserve<long long>((size_t)rows * P);
+    long long* idsrow = sg.reserve<long long>((size_t)B * ids_ld);
+    unsigned char* kv = sg.reserve<unsigned char>((size_t)rows * ids_ld);
+    int* leftpad = sg.reserve<int>(rows);
+    int* rowslot = sg.reserve<int>(rows);
+    unsigned char* vf = sg.reserve<unsigned char>(c.vocab_size_in);
+    GenState* gs = sg.reserve<GenState>(1);
+    SampleConfig* sc = sg.reserve<SampleConfig>(1);
+    MB_TRY(sg.fits());
+    MB_TRY(build_prompt_rows(m, rows, P, [&](int r) { return r % B; }, use_cfg ? B : 0, slots, prompt, prompt_mask, neg_prompt, neg_mask,
+                             pre, kv, leftpad, rowslot));
     for (int b = 0; b < B; ++b)
-        for (int t = 0; t < P; ++t) idsrow[(size_t)b * ids_ld + t] = prompt[(size_t)b * P + t];
-    GenState gs{};
-    gs.cur_len = P; gs.prompt_len = P; gs.max_length = gp->max_length; gs.min_new_tokens = gp->min_new_tokens;
-    const SampleConfig sc = make_sample_config(gp, B, use_cfg, V, ids_ld);
-
-    // The call state leaves from the engine's pinned staging buffer, so the copies are asynchronous and the prefill queues behind them
-    // with no host wait.  The buffer is refilled only once the previous call's copies completed (that call's closing sync normally
-    // saw to it; the event covers a call that returned early on an error).
-    MB_CUDA_CHECK(cudaEventSynchronize(m->stage_ev));
-    size_t stage_off = 0;
-    auto stage = [&](void* dst, const void* src, size_t n) -> int {
-        stage_off = (stage_off + 15) & ~size_t(15);
-        MB_REQUIRE(stage_off + n <= m->h_stage_bytes, "call state exceeds the staging buffer");
-        std::memcpy(m->h_stage + stage_off, src, n);
-        MB_CUDA_CHECK(cudaMemcpyAsync(dst, m->h_stage + stage_off, n, cudaMemcpyHostToDevice, st));
-        stage_off += n;
-        return 0;
-    };
-    MB_TRY(stage(m->g_prefill_ids.p, pre.data(), pre.size() * 8));
-    MB_TRY(stage(m->g_ids.p, idsrow.data(), idsrow.size() * 8));
-    MB_TRY(stage(m->g_keyvalid.p, kv.data(), kv.size()));
-    MB_TRY(stage(m->g_leftpad.p, leftpad.data(), rows * 4));
-    MB_TRY(stage(m->g_rowslot.p, rowslot.data(), rows * 4));
-    MB_TRY(stage(m->g_vflags.p, vflags, c.vocab_size_in));
-    MB_TRY(stage(m->g_state.p, &gs, sizeof(gs)));
-    MB_TRY(stage(m->g_cfg.p, &sc, sizeof(sc)));
-    MB_CUDA_CHECK(cudaEventRecord(m->stage_ev, st));
+        for (int t = 0; t < ids_ld; ++t) idsrow[(size_t)b * ids_ld + t] = t < P ? prompt[(size_t)b * P + t] : gp->pad_token_id;
+    std::memcpy(vf, vflags, c.vocab_size_in);
+    *gs = GenState{};
+    gs->cur_len = P; gs->prompt_len = P; gs->max_length = gp->max_length; gs->min_new_tokens = gp->min_new_tokens;
+    *sc = make_sample_config(gp, B, use_cfg, V, ids_ld);
+    MB_TRY(sg.upload(m->g_prefill_ids.p, pre, (size_t)rows * P));
+    MB_TRY(sg.upload(m->g_ids.p, idsrow, (size_t)B * ids_ld));
+    MB_TRY(sg.upload(m->g_keyvalid.p, kv, (size_t)rows * ids_ld));
+    MB_TRY(sg.upload(m->g_leftpad.p, leftpad, rows));
+    MB_TRY(sg.upload(m->g_rowslot.p, rowslot, rows));
+    MB_TRY(sg.upload(m->g_vflags.p, vf, c.vocab_size_in));
+    MB_TRY(sg.upload(m->g_state.p, gs, 1));
+    MB_TRY(sg.upload(m->g_cfg.p, sc, 1));
+    MB_TRY(sg.end());
     MB_CUDA_CHECK(cudaMemsetAsync(m->g_finished.p, 0, m->max_rows, st));
     MB_CUDA_CHECK(cudaMemsetAsync(m->d_ticket.p, 0, (size_t)m->max_rows * m->cfg.heads * sizeof(int), st));   // self-resetting; cleared in case a previous call aborted
 
-    // partial buffers for the split-KV attentions
-    const int chunk = 64;
     const int n_splits_self = self_splits(gp->max_length);
-    (void)H; (void)T;
-
-    MB_TRY(launch_prompt_scan(m->g_ids.as<long long>(), ids_ld, B, P, m->g_vflags.as<unsigned char>(), sc.ts_start, sc.ts_end,
+    MB_TRY(launch_prompt_scan(m->g_ids.as<long long>(), ids_ld, B, P, m->g_vflags.as<unsigned char>(), sc->ts_start, sc->ts_end,
                               m->g_lastts.as<int>(), st));
     // prefill + first token: ~230 small launches.  The first call of a given (rows, P) shape runs eagerly (it may allocate);
     // from the second call on the same sequence is replayed as one CUDA graph (sequential windows reuse a few prompt lengths).
@@ -985,29 +1043,16 @@ extern "C" int mb200_model_generate(mb200_model* m, const int32_t* slots, int32_
         } else {
             auto git = m->prefill_graphs.find(pkey);
             if (git == m->prefill_graphs.end()) {
-                if (!m->cap_stream) MB_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
-                MB_CUDA_CHECK(cudaStreamSynchronize(st));
-                cudaGraph_t graph;
-                MB_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
-                const long long before = g_launch_count;
-                int s = run_prefill(m->cap_stream);
-                cudaError_t e = cudaStreamEndCapture(m->cap_stream, &graph);
-                const long long nodes = g_launch_count - before;
-                g_launch_count = before;
-                if (s) return s;
-                MB_CUDA_CHECK(e);
-                cudaGraphExec_t exec;
-                MB_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
-                cudaGraphDestroy(graph);
+                CapturedGraph g;
+                MB_TRY(capture_graph(m->cap_stream, st, run_prefill, &g));
                 if (m->prefill_graphs.size() >= 48) {      // bounded cache: real songs see many prompt lengths; drop everything and re-learn
-                    for (auto& g : m->prefill_graphs) cudaGraphExecDestroy(g.second.first);
+                    for (auto& old : m->prefill_graphs) cudaGraphExecDestroy(old.second.exec);
                     m->prefill_graphs.clear();
                     m->prefill_seen.clear();
                 }
-                git = m->prefill_graphs.emplace(pkey, std::make_pair(exec, nodes)).first;
+                git = m->prefill_graphs.emplace(pkey, g).first;
             }
-            MB_CUDA_CHECK(cudaGraphLaunch(git->second.first, st));
-            g_launch_count += git->second.second;
+            MB_TRY(git->second.launch(st));
         }
     }
 
@@ -1045,37 +1090,12 @@ extern "C" int mb200_model_generate(mb200_model* m, const int32_t* slots, int32_
     auto key = std::make_tuple(rows, (int)B, n_splits_self, 1);
     auto it = m->graphs.find(key);
     if (it == m->graphs.end()) {
-        // capture on an engine-owned stream (the caller's stream may be the legacy default stream, which cannot capture)
-        cudaGraph_t graph;
-        if (!m->cap_stream) MB_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
-        MB_CUDA_CHECK(cudaStreamSynchronize(st));
-        MB_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
-        const long long before = g_launch_count;
-        int s = token_step(m, rows, B, n_splits_self, m->cap_stream, m->use_pdl);
-        cudaError_t e = cudaStreamEndCapture(m->cap_stream, &graph);
-        m->graph_nodes[key] = g_launch_count - before;
-        g_launch_count = before;   // captured, not launched; replays are counted below
-        if (s) return s;
-        MB_CUDA_CHECK(e);
-        cudaGraphExec_t exec;
-        MB_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
-        cudaGraphDestroy(graph);
-        it = m->graphs.emplace(key, exec).first;
+        CapturedGraph g;
+        MB_TRY(capture_graph(m->cap_stream, st, [&](cudaStream_t cs) { return token_step(m, rows, B, n_splits_self, cs, m->use_pdl); }, &g));
+        it = m->graphs.emplace(key, g).first;
     }
-    int remaining = gp->max_length - (P + 1);
-    const int burst_default = 16;
-    int produced = 1;
-    while (remaining > 0) {
-        int burst = std::min(remaining, burst_default);
-        // no EOS is possible before min_new_tokens are out, so the first poll can wait until then
-        if (gp->min_new_tokens > produced) burst = std::min(remaining, std::max(burst, gp->min_new_tokens - produced));
-        for (int i = 0; i < burst; ++i) MB_CUDA_CHECK(cudaGraphLaunch(it->second, st));
-        g_launch_count += (long long)burst * m->graph_nodes[key];
-        remaining -= burst; produced += burst;
-        MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag, &m->g_state.as<GenState>()->all_finished, 4, cudaMemcpyDeviceToHost, st));
-        MB_CUDA_CHECK(cudaStreamSynchronize(st));
-        if (*m->h_flag) break;
-    }
+    // no EOS is possible before min_new_tokens are out, so the first poll can wait until then
+    MB_TRY(replay_until_finished(m, it->second, gp->max_length - (P + 1), gp->min_new_tokens - 1, st));
     MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag, &m->g_state.as<GenState>()->cur_len, 4, cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
     const int L = *m->h_flag;
@@ -1097,8 +1117,7 @@ struct mb200_stream {
     mb200_model* m = nullptr;
     int N = 0, rows = 0, cap = 0;
     bool use_cfg = false;
-    cudaGraphExec_t step = nullptr;          // owned by m->graphs
-    long long step_nodes = 0;
+    CapturedGraph step;                      // the token-step graph; m->graphs owns its exec
     enum : int { FREE = 0, LIVE = 1, DONE = 2 };
     std::vector<int> status;                 // host view of each row
     std::vector<int> prompt_len, max_length, first_poll, selections;
@@ -1111,6 +1130,27 @@ namespace {
 void stream_release(mb200_stream* s) {
     if (s->h_rows) cudaFreeHost(s->h_rows);
     s->h_rows = nullptr;
+}
+
+// The host-side bounds of n ragged requests (a ragged call's or a stream admission's), checked before anything is launched: every
+// prompt 1 <= P < max_length <= cap, its encoder slot, guidance on every request or on none as the negative prompts say, its token ids.
+int check_requests(const mb200_model* m, int n, const int32_t* slots, const int64_t* prompt, const int32_t* prompt_off,
+                   const int64_t* neg_prompt, const mb200_generate_params* params, int cap) {
+    const auto& c = m->cfg;
+    MB_REQUIRE(prompt_off[0] == 0, "prompt offsets start at 0");
+    for (int j = 0; j < n; ++j) {
+        const mb200_generate_params& gp = params[j];
+        const int P = prompt_off[j + 1] - prompt_off[j];
+        MB_REQUIRE(P >= 1 && P < gp.max_length && gp.max_length <= cap,
+                   "need 1 <= prompt_len < max_length <= the max_length cap (tgt_seq_len, or a stream's own) for every request");
+        MB_REQUIRE(slots[j] >= 0 && slots[j] < c.max_windows, "encoder slot out of range");
+        MB_REQUIRE((gp.cfg_scale > 1.0f) == (neg_prompt != nullptr), "classifier-free guidance on every request or on none");
+        for (int t = prompt_off[j]; t < prompt_off[j + 1]; ++t) {
+            MB_REQUIRE(prompt[t] >= 0 && prompt[t] < c.vocab_size_in, "prompt token id out of range");
+            MB_REQUIRE(!neg_prompt || (neg_prompt[t] >= 0 && neg_prompt[t] < c.vocab_size_in), "negative prompt token id out of range");
+        }
+    }
+    return 0;
 }
 
 // Fixes the shape (capacity N, guidance, max_length cap), captures the ragged step graph of (rows, N, self_splits(cap)) if this engine
@@ -1147,23 +1187,13 @@ int stream_open(mb200_model* m, mb200_stream* s, int N, bool use_cfg, int cap, c
     auto key = std::make_tuple(rows, N, self_splits(cap), -1);
     auto it = m->graphs.find(key);
     if (it == m->graphs.end()) {
-        cudaGraph_t graph;
-        if (!m->cap_stream) MB_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
-        MB_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
-        const long long before = g_launch_count;
-        int e1 = token_step(m, rows, N, self_splits(cap), m->cap_stream, m->use_pdl, nullptr, nullptr, true);
-        cudaError_t e = cudaStreamEndCapture(m->cap_stream, &graph);
-        m->graph_nodes[key] = g_launch_count - before;
-        g_launch_count = before;
-        if (e1) return e1;
-        MB_CUDA_CHECK(e);
-        cudaGraphExec_t exec;
-        MB_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
-        cudaGraphDestroy(graph);
-        it = m->graphs.emplace(key, exec).first;
+        CapturedGraph g;
+        MB_TRY(capture_graph(m->cap_stream, st, [&](cudaStream_t cs) {
+            return token_step(m, rows, N, self_splits(cap), cs, m->use_pdl, nullptr, nullptr, true);
+        }, &g));
+        it = m->graphs.emplace(key, g).first;
     }
     s->step = it->second;
-    s->step_nodes = m->graph_nodes[key];
     return 0;
 }
 
@@ -1175,55 +1205,30 @@ int stream_admit(mb200_stream* s, int n, const int32_t* slots, const int64_t* pr
     mb200_model* m = s->m;
     const auto& c = m->cfg;
     MB_REQUIRE(slots && prompt && prompt_off && vflags && params && rows_out, "null argument");
-    MB_REQUIRE(prompt_off[0] == 0, "prompt offsets start at 0");
     MB_REQUIRE((neg_prompt != nullptr) == s->use_cfg, "a negative prompt with every request of a guided stream and with none of an unguided one");
     std::vector<int> free_rows;
     for (int r = 0; r < s->N; ++r) if (s->status[r] == mb200_stream::FREE) free_rows.push_back(r);
     MB_REQUIRE(n >= 1 && n <= (int)free_rows.size(), "the stream has fewer free rows than requests to admit");
+    MB_TRY(check_requests(m, n, slots, prompt, prompt_off, neg_prompt, params, s->cap));
     const int d = c.d_model, V = c.vocab_size_out, ids_ld = c.tgt_seq_len, Vin = c.vocab_size_in, N = s->N, nr = s->use_cfg ? 2 : 1;
-    for (int j = 0; j < n; ++j) {
-        const mb200_generate_params& gp = params[j];
-        const int P = prompt_off[j + 1] - prompt_off[j];
-        MB_REQUIRE(P >= 1 && P < gp.max_length && gp.max_length <= s->cap, "need 1 <= prompt_len < max_length <= the stream's max_length cap for every request");
-        MB_REQUIRE(slots[j] >= 0 && slots[j] < c.max_windows, "encoder slot out of range");
-        MB_REQUIRE((gp.cfg_scale > 1.0f) == s->use_cfg, "classifier-free guidance on every request of a stream or on none");
-        for (int t = prompt_off[j]; t < prompt_off[j + 1]; ++t) {
-            MB_REQUIRE(prompt[t] >= 0 && prompt[t] < Vin, "prompt token id out of range");
-            MB_REQUIRE(!neg_prompt || (neg_prompt[t] >= 0 && neg_prompt[t] < Vin), "negative prompt token id out of range");
-        }
-    }
     // ---- staging ----
-    MB_CUDA_CHECK(cudaEventSynchronize(m->stage_ev));       // the previous admission's copies left the pinned buffer
-    size_t stage_off = 0;
-    auto stage = [&](size_t n_bytes) -> void* {
-        stage_off = (stage_off + 15) & ~size_t(15);
-        if (stage_off + n_bytes > m->h_stage_bytes) return nullptr;
-        void* h = m->h_stage + stage_off;
-        stage_off += n_bytes;
-        return h;
-    };
-    auto copy = [&](void* dst, const void* h, size_t n_bytes) -> int {
-        MB_CUDA_CHECK(cudaMemcpyAsync(dst, h, n_bytes, cudaMemcpyHostToDevice, st));
-        return 0;
-    };
-    int* list = static_cast<int*>(stage((size_t)n * sizeof(int)));
-    MB_REQUIRE(list, "admission exceeds the staging buffer");
+    Stager sg{m, st};
+    MB_TRY(sg.begin());
+    int* list = sg.reserve<int>(n);
     std::vector<size_t> pre_off(n);
     size_t total = 0;
     for (int j = 0; j < n; ++j) { pre_off[j] = total; total += (size_t)nr * (prompt_off[j + 1] - prompt_off[j]); }
-    long long* pre = static_cast<long long*>(stage(total * 8));
-    MB_REQUIRE(pre, "admission exceeds the staging buffer");
-    // pointers into the pinned buffer for every per-row record; checked all at once before the first copy is issued
+    long long* pre = sg.reserve<long long>(total);
     std::vector<long long*> h_ids(n); std::vector<RowState*> h_rs(n); std::vector<SampleConfig*> h_cfg(n); std::vector<int*> h_slot(n);
     std::vector<unsigned char*> h_vf(n);
     for (int j = 0; j < n; ++j) {
-        h_ids[j] = static_cast<long long*>(stage((size_t)ids_ld * 8));
-        h_rs[j] = static_cast<RowState*>(stage(sizeof(RowState)));
-        h_cfg[j] = static_cast<SampleConfig*>(stage(sizeof(SampleConfig)));
-        h_vf[j] = static_cast<unsigned char*>(stage((size_t)Vin));
-        h_slot[j] = static_cast<int*>(stage(4 * sizeof(int)));
-        MB_REQUIRE(h_ids[j] && h_rs[j] && h_cfg[j] && h_vf[j] && h_slot[j], "admission exceeds the staging buffer");
+        h_ids[j] = sg.reserve<long long>(ids_ld);
+        h_rs[j] = sg.reserve<RowState>(1);
+        h_cfg[j] = sg.reserve<SampleConfig>(1);
+        h_vf[j] = sg.reserve<unsigned char>(Vin);
+        h_slot[j] = sg.reserve<int>(4);
     }
+    MB_TRY(sg.fits());
     for (int j = 0; j < n; ++j) {
         const mb200_generate_params& gp = params[j];
         const int P = prompt_off[j + 1] - prompt_off[j], r = free_rows[j];
@@ -1243,18 +1248,18 @@ int stream_admit(mb200_stream* s, int n, const int32_t* slots, const int64_t* pr
     GenState* gs = m->g_state.as<GenState>();
     int* rowslot = m->g_rowslot.as<int>();
     int* d_list = rowslot + 3 * m->max_rows;
-    MB_TRY(copy(d_list, list, (size_t)n * sizeof(int)));
-    MB_TRY(copy(m->g_prefill_ids.p, pre, total * 8));
+    MB_TRY(sg.upload(d_list, list, n));
+    MB_TRY(sg.upload(m->g_prefill_ids.p, pre, total));
     for (int j = 0; j < n; ++j) {
         const int r = list[j];
-        MB_TRY(copy(m->g_ids.as<long long>() + (size_t)r * ids_ld, h_ids[j], (size_t)ids_ld * 8));
-        MB_TRY(copy(ragged_rows(gs) + r, h_rs[j], sizeof(RowState)));
-        MB_TRY(copy(m->g_cfg.as<SampleConfig>() + r, h_cfg[j], sizeof(SampleConfig)));
-        MB_TRY(copy(m->g_vflags.as<unsigned char>() + (size_t)r * Vin, h_vf[j], (size_t)Vin));
-        for (int i = 0; i < nr; ++i) MB_TRY(copy(rowslot + r + i * N, h_slot[j], sizeof(int)));      // decode rows r, N + r
-        MB_TRY(copy(rowslot + m->max_rows + 2 * r, h_slot[j], 2 * sizeof(int)));                     // the prefill's (slot, slot) pair
+        MB_TRY(sg.upload(m->g_ids.as<long long>() + (size_t)r * ids_ld, h_ids[j], ids_ld));
+        MB_TRY(sg.upload(ragged_rows(gs) + r, h_rs[j], 1));
+        MB_TRY(sg.upload(m->g_cfg.as<SampleConfig>() + r, h_cfg[j], 1));
+        MB_TRY(sg.upload(m->g_vflags.as<unsigned char>() + (size_t)r * Vin, h_vf[j], Vin));
+        for (int i = 0; i < nr; ++i) MB_TRY(sg.upload(rowslot + r + i * N, h_slot[j], 1));      // decode rows r, N + r
+        MB_TRY(sg.upload(rowslot + m->max_rows + 2 * r, h_slot[j], 2));                         // the prefill's (slot, slot) pair
     }
-    MB_CUDA_CHECK(cudaEventRecord(m->stage_ev, st));
+    MB_TRY(sg.end());
     for (int j = 0; j < n; ++j) {
         const int r = list[j];
         s->status[r] = mb200_stream::LIVE;
@@ -1299,8 +1304,7 @@ int stream_run(mb200_stream* s, int waiting, int32_t* done_rows, int32_t* done_l
     }
     if (!live) return 0;
     const int burst = std::max(0, std::min(remaining, std::max(waiting > 0 ? 2 : 16, earliest)));
-    for (int i = 0; i < burst; ++i) MB_CUDA_CHECK(cudaGraphLaunch(s->step, st));
-    g_launch_count += (long long)burst * s->step_nodes;
+    MB_TRY(s->step.launch(st, burst));
     *steps = burst;
     MB_CUDA_CHECK(cudaMemcpyAsync(s->h_rows, ragged_rows(m->g_state.as<GenState>()), (size_t)s->N * sizeof(RowState), cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -1375,27 +1379,17 @@ extern "C" int mb200_model_generate_ragged(mb200_model* m, int32_t n_req, const 
                                            const int64_t* neg_prompt, const uint8_t* vflags, const mb200_generate_params* params,
                                            int64_t* out_ids, int32_t out_ld, int32_t* out_len, void* stream) {
     MB_REQUIRE(m && m->finalized, "model not finalized");
-    MB_REQUIRE(!m->live_stream, "a decode stream is open on this engine: close it first");
+    MB_TRY(token_loop_free(m));
     MB_REQUIRE(slots && prompt && prompt_off && vflags && params && out_ids && out_len, "null argument");
-    const auto& c = m->cfg;
     cudaStream_t st = (cudaStream_t)stream;
     const bool use_cfg = neg_prompt != nullptr;
     const int N = n_req;
     MB_REQUIRE(N >= 1 && (use_cfg ? 2 * N : N) <= m->max_rows, "requests exceed max_batch (rows double under classifier-free guidance)");
-    MB_REQUIRE(prompt_off[0] == 0, "prompt offsets start at 0");
+    MB_TRY(check_requests(m, N, slots, prompt, prompt_off, neg_prompt, params, m->cfg.tgt_seq_len));
     int cap = 2;
     for (int r = 0; r < N; ++r) {
-        const mb200_generate_params& gp = params[r];
-        const int P = prompt_off[r + 1] - prompt_off[r];
-        MB_REQUIRE(P >= 1 && P < gp.max_length && gp.max_length <= c.tgt_seq_len, "need 1 <= prompt_len < max_length <= tgt_seq_len for every request");
-        MB_REQUIRE(gp.max_length <= out_ld, "output rows are shorter than a request's max_length");
-        MB_REQUIRE(slots[r] >= 0 && slots[r] < c.max_windows, "encoder slot out of range");
-        MB_REQUIRE((gp.cfg_scale > 1.0f) == use_cfg, "classifier-free guidance on every request of a ragged call or on none");
-        for (int t = prompt_off[r]; t < prompt_off[r + 1]; ++t) {
-            MB_REQUIRE(prompt[t] >= 0 && prompt[t] < c.vocab_size_in, "prompt token id out of range");
-            MB_REQUIRE(!use_cfg || (neg_prompt[t] >= 0 && neg_prompt[t] < c.vocab_size_in), "negative prompt token id out of range");
-        }
-        cap = std::max(cap, (int)gp.max_length);
+        MB_REQUIRE(params[r].max_length <= out_ld, "output rows are shorter than a request's max_length");
+        cap = std::max(cap, (int)params[r].max_length);
     }
     mb200_stream s;
     int e = stream_open(m, &s, N, use_cfg, cap, st);
@@ -1453,7 +1447,7 @@ extern "C" int mb200_model_generate_beams(mb200_model* m, const int32_t* slots, 
                                           const mb200_generate_params* gp, int32_t num_beams, int64_t fill_id, int64_t* out_ids,
                                           int32_t* out_len, float* out_scores, void* stream) {
     MB_REQUIRE(m && m->finalized, "model not finalized");
-    MB_REQUIRE(!m->live_stream, "a decode stream is open on this engine: close it first");
+    MB_TRY(token_loop_free(m));
     MB_REQUIRE(slots && prompt && vflags && gp && out_ids && out_len && out_scores, "null argument");
     const auto& c = m->cfg;
     cudaStream_t st = (cudaStream_t)stream;
@@ -1464,61 +1458,59 @@ extern "C" int mb200_model_generate_beams(mb200_model* m, const int32_t* slots, 
     const int BK = B * K, rows = use_cfg ? 2 * BK : BK;
     MB_REQUIRE(B >= 1 && rows <= m->max_rows, "batch * num_beams (x2 under classifier-free guidance) exceeds max_batch");
     MB_REQUIRE(P >= 1 && P < gp->max_length && gp->max_length <= c.tgt_seq_len, "need 1 <= prompt_len < max_length <= tgt_seq_len");
-    for (int b = 0; b < B; ++b) MB_REQUIRE(slots[b] >= 0 && slots[b] < c.max_windows, "encoder slot out of range");
     const int d = c.d_model, V = c.vocab_size_out, ids_ld = c.tgt_seq_len;
     MB_REQUIRE(beam_select_smem_bytes(K, V, ids_ld) <= 220 * 1024, "beam candidates do not fit shared memory");
     MB_TRY(ensure_beam_buffers(m));
 
-    // ---- host staging: row r is beam (r mod B*K) % K of item (r mod B*K) / K; rows [0, B*K) carry the negative prompt under CFG ----
-    std::vector<long long> pre((size_t)rows * P), idsrow((size_t)BK * ids_ld, (long long)gp->pad_token_id);
-    std::vector<unsigned char> kv((size_t)rows * ids_ld, 1);
-    std::vector<int> leftpad(rows, 0), rowslot(rows), kvsrc((size_t)rows * ids_ld, 0);
-    for (int r = 0; r < rows; ++r) {
-        const int b = (r % BK) / K;
-        const bool neg_row = use_cfg && r < BK;
-        const int64_t* src = neg_row ? neg_prompt : prompt;
-        const uint8_t* msk = neg_row ? (neg_mask ? neg_mask : prompt_mask) : prompt_mask;
-        int npad = 0; bool seen = false;
-        for (int t = 0; t < P; ++t) {
-            long long tok = src[(size_t)b * P + t];
-            MB_REQUIRE(tok >= 0 && tok < c.vocab_size_in, "prompt token id out of range");
-            pre[(size_t)r * P + t] = tok;
-            unsigned char ok = msk ? (msk[(size_t)b * P + t] != 0) : 1;
-            kv[(size_t)r * ids_ld + t] = ok;
-            if (!ok && !seen) ++npad; else seen = true;
-            kvsrc[(size_t)r * ids_ld + t] = r;
-        }
-        leftpad[r] = npad;
-        rowslot[r] = slots[b];
-    }
+    // ---- call state: row r is beam (r mod B*K) % K of item (r mod B*K) / K; rows [0, B*K) carry the negative prompt under CFG ----
+    Stager sg{m, st};
+    MB_TRY(sg.begin());
+    long long* pre = sg.reserve<long long>((size_t)rows * P);
+    long long* idsrow = sg.reserve<long long>((size_t)BK * ids_ld);
+    unsigned char* kv = sg.reserve<unsigned char>((size_t)rows * ids_ld);
+    int* leftpad = sg.reserve<int>(rows);
+    int* rowslot = sg.reserve<int>(rows);
+    unsigned char* vf = sg.reserve<unsigned char>(c.vocab_size_in);
+    GenState* gs = sg.reserve<GenState>(1);
+    SampleConfig* sc = sg.reserve<SampleConfig>(1);
+    int* kvsrc = sg.reserve<int>((size_t)rows * ids_ld);
+    float* runscore = sg.reserve<float>(BK);
+    float* finscore = sg.reserve<float>(BK);
+    MB_TRY(sg.fits());
+    MB_TRY(build_prompt_rows(m, rows, P, [&](int r) { return (r % BK) / K; }, use_cfg ? BK : 0, slots, prompt, prompt_mask, neg_prompt,
+                             neg_mask, pre, kv, leftpad, rowslot));
+    for (int r = 0; r < rows; ++r)      // every row reads its own prompt keys
+        for (int t = 0; t < ids_ld; ++t) kvsrc[(size_t)r * ids_ld + t] = t < P ? r : 0;
     for (int j = 0; j < BK; ++j)
-        for (int t = 0; t < P; ++t) idsrow[(size_t)j * ids_ld + t] = prompt[(size_t)(j / K) * P + t];
-    std::vector<float> runscore(BK), finscore(BK, -1.0e9f);
-    for (int j = 0; j < BK; ++j) runscore[j] = j % K == 0 ? 0.f : -1.0e9f;
-    GenState gs{};
-    gs.cur_len = P; gs.prompt_len = P; gs.max_length = gp->max_length; gs.min_new_tokens = gp->min_new_tokens;
-    const SampleConfig sc = make_sample_config(gp, BK, use_cfg, V, ids_ld);
-
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_prefill_ids.p, pre.data(), pre.size() * 8, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_ids.p, idsrow.data(), idsrow.size() * 8, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_keyvalid.p, kv.data(), kv.size(), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_leftpad.p, leftpad.data(), rows * 4, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_rowslot.p, rowslot.data(), rows * 4, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_vflags.p, vflags, c.vocab_size_in, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_state.p, &gs, sizeof(gs), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_cfg.p, &sc, sizeof(sc), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->b_kvsrc.p, kvsrc.data(), kvsrc.size() * 4, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->b_runscore.p, runscore.data(), BK * 4, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->b_finscore.p, finscore.data(), BK * 4, cudaMemcpyHostToDevice, st));
+        for (int t = 0; t < ids_ld; ++t) idsrow[(size_t)j * ids_ld + t] = t < P ? prompt[(size_t)(j / K) * P + t] : gp->pad_token_id;
+    for (int j = 0; j < BK; ++j) {
+        runscore[j] = j % K == 0 ? 0.f : -1.0e9f;
+        finscore[j] = -1.0e9f;
+    }
+    std::memcpy(vf, vflags, c.vocab_size_in);
+    *gs = GenState{};
+    gs->cur_len = P; gs->prompt_len = P; gs->max_length = gp->max_length; gs->min_new_tokens = gp->min_new_tokens;
+    *sc = make_sample_config(gp, BK, use_cfg, V, ids_ld);
+    MB_TRY(sg.upload(m->g_prefill_ids.p, pre, (size_t)rows * P));
+    MB_TRY(sg.upload(m->g_ids.p, idsrow, (size_t)BK * ids_ld));
+    MB_TRY(sg.upload(m->g_keyvalid.p, kv, (size_t)rows * ids_ld));
+    MB_TRY(sg.upload(m->g_leftpad.p, leftpad, rows));
+    MB_TRY(sg.upload(m->g_rowslot.p, rowslot, rows));
+    MB_TRY(sg.upload(m->g_vflags.p, vf, c.vocab_size_in));
+    MB_TRY(sg.upload(m->g_state.p, gs, 1));
+    MB_TRY(sg.upload(m->g_cfg.p, sc, 1));
+    MB_TRY(sg.upload(m->b_kvsrc.p, kvsrc, (size_t)rows * ids_ld));
+    MB_TRY(sg.upload(m->b_runscore.p, runscore, BK));
+    MB_TRY(sg.upload(m->b_finscore.p, finscore, BK));
+    MB_TRY(sg.end());
     MB_CUDA_CHECK(cudaMemsetAsync(m->b_finlen.p, 0, BK * sizeof(int), st));
     MB_CUDA_CHECK(cudaMemsetAsync(m->b_finflag.p, 0, BK, st));
     MB_CUDA_CHECK(cudaMemsetAsync(m->b_unsat.p, 1, B, st));
     MB_CUDA_CHECK(cudaMemsetAsync(m->d_ticket.p, 0, (size_t)m->max_rows * m->cfg.heads * sizeof(int), st));
-    MB_CUDA_CHECK(cudaStreamSynchronize(st));   // host vectors go out of scope; the copies above are from pageable memory
 
     const BeamParams bp = beam_params(m, rows, K);
 
-    MB_TRY(launch_prompt_scan(m->g_ids.as<long long>(), ids_ld, BK, P, m->g_vflags.as<unsigned char>(), sc.ts_start, sc.ts_end,
+    MB_TRY(launch_prompt_scan(m->g_ids.as<long long>(), ids_ld, BK, P, m->g_vflags.as<unsigned char>(), sc->ts_start, sc->ts_end,
                               m->g_lastts.as<int>(), st));
     MB_TRY(decoder_prefill(m, rows, P, m->g_prefill_ids.as<long long>(), gp->position_rule, st));
     MB_TRY(final_logits(m, rows, m->p_x.as<float>() + (size_t)(P - 1) * d, (long long)P * d, st, false));
@@ -1528,44 +1520,26 @@ extern "C" int mb200_model_generate_beams(mb200_model* m, const int32_t* slots, 
     auto key = std::make_tuple(rows, (int)B, n_splits_self, K);
     auto it = m->graphs.find(key);
     if (it == m->graphs.end()) {
-        cudaGraph_t graph;
-        if (!m->cap_stream) MB_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
-        MB_CUDA_CHECK(cudaStreamSynchronize(st));
-        MB_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
-        const long long before = g_launch_count;
-        int s = token_step(m, rows, B, n_splits_self, m->cap_stream, m->use_pdl, nullptr, &bp);
-        cudaError_t e = cudaStreamEndCapture(m->cap_stream, &graph);
-        m->graph_nodes[key] = g_launch_count - before;
-        g_launch_count = before;
-        if (s) return s;
-        MB_CUDA_CHECK(e);
-        cudaGraphExec_t exec;
-        MB_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
-        cudaGraphDestroy(graph);
-        it = m->graphs.emplace(key, exec).first;
+        CapturedGraph g;
+        MB_TRY(capture_graph(m->cap_stream, st, [&](cudaStream_t cs) { return token_step(m, rows, B, n_splits_self, cs, m->use_pdl, nullptr, &bp); },
+                             &g));
+        it = m->graphs.emplace(key, g).first;
     }
     int remaining = gp->max_length - (P + 1);
     MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag, &m->g_state.as<GenState>()->all_finished, 4, cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
     if (*m->h_flag) remaining = 0;
-    while (remaining > 0) {
-        const int burst = std::min(remaining, 16);
-        for (int i = 0; i < burst; ++i) MB_CUDA_CHECK(cudaGraphLaunch(it->second, st));
-        g_launch_count += (long long)burst * m->graph_nodes[key];
-        remaining -= burst;
-        MB_CUDA_CHECK(cudaMemcpyAsync(m->h_flag, &m->g_state.as<GenState>()->all_finished, 4, cudaMemcpyDeviceToHost, st));
-        MB_CUDA_CHECK(cudaStreamSynchronize(st));
-        if (*m->h_flag) break;
-    }
+    MB_TRY(replay_until_finished(m, it->second, remaining, 0, st));
     GenState fin{};
     MB_CUDA_CHECK(cudaMemcpyAsync(&fin, m->g_state.p, sizeof(fin), cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
     // the finished store the last selection wrote (parity of the step count)
     std::vector<long long> fids((size_t)BK * ids_ld);
+    std::vector<float> fscore(BK);
     std::vector<int> flen(BK);
     std::vector<unsigned char> fflag(BK);
     MB_CUDA_CHECK(cudaMemcpyAsync(fids.data(), m->b_finids[fin.step & 1].p, fids.size() * 8, cudaMemcpyDeviceToHost, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(finscore.data(), m->b_finscore.p, BK * 4, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(fscore.data(), m->b_finscore.p, BK * 4, cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaMemcpyAsync(flen.data(), m->b_finlen.p, BK * 4, cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaMemcpyAsync(fflag.data(), m->b_finflag.p, BK, cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -1580,7 +1554,7 @@ extern "C" int mb200_model_generate_beams(mb200_model* m, const int32_t* slots, 
         const long long* h = fids.data() + (size_t)b * K * ids_ld;
         const int Lb = P + flen[(size_t)b * K];
         for (int t = 0; t < Lout; ++t) out_ids[(size_t)b * Lout + t] = t < Lb ? h[t] : fill_id;
-        out_scores[b] = finscore[(size_t)b * K];
+        out_scores[b] = fscore[(size_t)b * K];
     }
     *out_len = Lout;
     return 0;
@@ -1591,30 +1565,23 @@ extern "C" int mb200_model_generate_beams(mb200_model* m, const int32_t* slots, 
 static int teacher_forced_hidden(mb200_model* m, const int32_t* slots, int32_t B, const int64_t* ids, const uint8_t* mask, int32_t len,
                                  int32_t position_rule, cudaStream_t st) {
     MB_REQUIRE(m && m->finalized, "model not finalized");
-    MB_REQUIRE(!m->live_stream, "a decode stream is open on this engine: close it first");
+    MB_TRY(token_loop_free(m));
     MB_REQUIRE(B >= 1 && B <= m->max_rows && len >= 1 && len <= m->cfg.tgt_seq_len, "bad batch / length");
     const auto& c = m->cfg;
     const int ids_ld = c.tgt_seq_len, d = c.d_model;
-    std::vector<unsigned char> kv((size_t)B * ids_ld, 1);
-    std::vector<int> leftpad(B, 0), rowslot(B);
-    std::vector<long long> pre((size_t)B * len);
-    for (int b = 0; b < B; ++b) {
-        int npad = 0; bool seen = false;
-        for (int t = 0; t < len; ++t) {
-            long long tok = ids[(size_t)b * len + t];
-            MB_REQUIRE(tok >= 0 && tok < c.vocab_size_in, "token id out of range");
-            pre[(size_t)b * len + t] = tok;
-            unsigned char ok = mask ? (mask[(size_t)b * len + t] != 0) : 1;
-            kv[(size_t)b * ids_ld + t] = ok;
-            if (!ok && !seen) ++npad; else seen = true;
-        }
-        leftpad[b] = npad; rowslot[b] = slots[b];
-    }
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_prefill_ids.p, pre.data(), pre.size() * 8, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_keyvalid.p, kv.data(), kv.size(), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_leftpad.p, leftpad.data(), B * 4, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_rowslot.p, rowslot.data(), B * 4, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaStreamSynchronize(st));
+    Stager sg{m, st};
+    MB_TRY(sg.begin());
+    long long* pre = sg.reserve<long long>((size_t)B * len);
+    unsigned char* kv = sg.reserve<unsigned char>((size_t)B * ids_ld);
+    int* leftpad = sg.reserve<int>(B);
+    int* rowslot = sg.reserve<int>(B);
+    MB_TRY(sg.fits());
+    MB_TRY(build_prompt_rows(m, B, len, [](int r) { return r; }, 0, slots, ids, mask, nullptr, nullptr, pre, kv, leftpad, rowslot));
+    MB_TRY(sg.upload(m->g_prefill_ids.p, pre, (size_t)B * len));
+    MB_TRY(sg.upload(m->g_keyvalid.p, kv, (size_t)B * ids_ld));
+    MB_TRY(sg.upload(m->g_leftpad.p, leftpad, B));
+    MB_TRY(sg.upload(m->g_rowslot.p, rowslot, B));
+    MB_TRY(sg.end());
     MB_TRY(decoder_prefill(m, B, len, m->g_prefill_ids.as<long long>(), position_rule, st));
     MB_TRY(layernorm(m->p_x.as<float>(), m->p_h.as<float>(), m->dec_ln_w, m->dec_ln_b, B * len, d, 1e-5f, st));
     return 0;
@@ -1667,8 +1634,9 @@ extern "C" int mb200_model_score_tokens(mb200_model* m, const int32_t* slots, in
 extern "C" int mb200_model_set_option(mb200_model* m, const char* name, int value) {
     MB_REQUIRE(m && name, "null argument");
     if (!strcmp(name, "pdl")) {
+        MB_TRY(token_loop_free(m));      // the toggle destroys every token-step graph, the open stream's among them
         if (m->use_pdl != (value != 0)) {
-            for (auto& g : m->graphs) cudaGraphExecDestroy(g.second);
+            for (auto& g : m->graphs) cudaGraphExecDestroy(g.second.exec);
             m->graphs.clear();
         }
         m->use_pdl = value != 0;
@@ -1697,6 +1665,7 @@ extern "C" int mb200_model_set_option(mb200_model* m, const char* name, int valu
 // spent in {gemv, split-KV attention, logits/sample} kernels, out_us[3] = their launch counts packed as gemv*1e6 + attn*1e3 + sample.
 extern "C" int mb200_model_profile_step(mb200_model* m, int32_t rows, int32_t B, int32_t max_length, int32_t iters, float* out_us, void* stream) {
     MB_REQUIRE(m && m->finalized && out_us && iters >= 1, "bad argument");
+    MB_TRY(token_loop_free(m));
     cudaStream_t st = (cudaStream_t)stream;
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
     GenState gs{};
@@ -1751,27 +1720,34 @@ extern "C" int mb200_model_logits_chain(mb200_model* m, const float* logits, int
                                         int32_t prompt_len, const uint8_t* vflags, const mb200_generate_params* gp, int32_t step,
                                         int32_t has_last_scores, float* scores_out, int64_t* chosen_out, void* stream) {
     MB_REQUIRE(m && m->finalized && logits && ids && vflags && gp && scores_out && chosen_out, "null argument");
+    MB_TRY(token_loop_free(m));
     const auto& c = m->cfg;
     const int rows = use_cfg ? 2 * B : B, V = c.vocab_size_out, ids_ld = c.tgt_seq_len;
     MB_REQUIRE(B >= 1 && rows <= m->max_rows && L >= 1 && L < ids_ld, "bad batch / length");
     cudaStream_t st = (cudaStream_t)stream;
-    std::vector<long long> idsrow((size_t)B * ids_ld, (long long)gp->pad_token_id);
+    Stager sg{m, st};
+    MB_TRY(sg.begin());
+    long long* idsrow = sg.reserve<long long>((size_t)B * ids_ld);
+    unsigned char* vf = sg.reserve<unsigned char>(c.vocab_size_in);
+    GenState* gs = sg.reserve<GenState>(1);
+    SampleConfig* sc = sg.reserve<SampleConfig>(1);
+    MB_TRY(sg.fits());
     for (int b = 0; b < B; ++b)
-        for (int t = 0; t < L; ++t) idsrow[(size_t)b * ids_ld + t] = ids[(size_t)b * L + t];
-    GenState gs{};
-    gs.cur_len = L; gs.prompt_len = prompt_len; gs.max_length = gp->max_length; gs.min_new_tokens = gp->min_new_tokens;
-    gs.step = step; gs.has_last_scores = has_last_scores;
-    const SampleConfig sc = make_sample_config(gp, B, use_cfg != 0, V, ids_ld);
-    std::vector<int> zeros(rows, 0);
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_ids.p, idsrow.data(), idsrow.size() * 8, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_vflags.p, vflags, c.vocab_size_in, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_state.p, &gs, sizeof(gs), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_cfg.p, &sc, sizeof(sc), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_leftpad.p, zeros.data(), rows * 4, cudaMemcpyHostToDevice, st));
+        for (int t = 0; t < ids_ld; ++t) idsrow[(size_t)b * ids_ld + t] = t < L ? ids[(size_t)b * L + t] : gp->pad_token_id;
+    std::memcpy(vf, vflags, c.vocab_size_in);
+    *gs = GenState{};
+    gs->cur_len = L; gs->prompt_len = prompt_len; gs->max_length = gp->max_length; gs->min_new_tokens = gp->min_new_tokens;
+    gs->step = step; gs->has_last_scores = has_last_scores;
+    *sc = make_sample_config(gp, B, use_cfg != 0, V, ids_ld);
+    MB_TRY(sg.upload(m->g_ids.p, idsrow, (size_t)B * ids_ld));
+    MB_TRY(sg.upload(m->g_vflags.p, vf, c.vocab_size_in));
+    MB_TRY(sg.upload(m->g_state.p, gs, 1));
+    MB_TRY(sg.upload(m->g_cfg.p, sc, 1));
+    MB_TRY(sg.end());
+    MB_CUDA_CHECK(cudaMemsetAsync(m->g_leftpad.p, 0, rows * sizeof(int), st));
     MB_CUDA_CHECK(cudaMemsetAsync(m->g_finished.p, 0, m->max_rows, st));
     MB_CUDA_CHECK(cudaMemcpyAsync(m->d_logits.p, logits, (size_t)rows * V * 4, cudaMemcpyDeviceToDevice, st));
-    MB_CUDA_CHECK(cudaStreamSynchronize(st));
-    MB_TRY(launch_prompt_scan(m->g_ids.as<long long>(), ids_ld, B, L, m->g_vflags.as<unsigned char>(), sc.ts_start, sc.ts_end, m->g_lastts.as<int>(), st));
+    MB_TRY(launch_prompt_scan(m->g_ids.as<long long>(), ids_ld, B, L, m->g_vflags.as<unsigned char>(), sc->ts_start, sc->ts_end, m->g_lastts.as<int>(), st));
     SampleParams sp = sample_params(m, rows);
     sp.dbg_scores = scores_out;
     MB_TRY(launch_sample(sp, B, st, false));
@@ -1796,6 +1772,7 @@ extern "C" int mb200_model_beam_step(mb200_model* m, const float* logits, int32_
                                      uint8_t* fin_flag_out, int64_t* fin_ids_out, void* stream) {
     MB_REQUIRE(m && m->finalized && logits && ids && vflags && gp && run_scores && logprobs_out && top_out && parent_out && token_out &&
                score_out && fin_score_out && fin_len_out && fin_flag_out && fin_ids_out, "null argument");
+    MB_TRY(token_loop_free(m));
     const auto& c = m->cfg;
     const int K = num_beams, BK = B * K, rows = use_cfg ? 2 * BK : BK, V = c.vocab_size_out, ids_ld = c.tgt_seq_len;
     MB_REQUIRE(K >= 2 && K <= 4, "num_beams must be in [2, 4]");
@@ -1803,29 +1780,38 @@ extern "C" int mb200_model_beam_step(mb200_model* m, const float* logits, int32_
     MB_REQUIRE(beam_select_smem_bytes(K, V, ids_ld) <= 220 * 1024, "beam candidates do not fit shared memory");
     cudaStream_t st = (cudaStream_t)stream;
     MB_TRY(ensure_beam_buffers(m));
-    std::vector<long long> idsrow((size_t)BK * ids_ld, (long long)gp->pad_token_id);
+    Stager sg{m, st};
+    MB_TRY(sg.begin());
+    long long* idsrow = sg.reserve<long long>((size_t)BK * ids_ld);
+    unsigned char* vf = sg.reserve<unsigned char>(c.vocab_size_in);
+    GenState* gs = sg.reserve<GenState>(1);
+    SampleConfig* sc = sg.reserve<SampleConfig>(1);
+    float* runscore = sg.reserve<float>(BK);
+    float* finscore = sg.reserve<float>(BK);
+    MB_TRY(sg.fits());
     for (int j = 0; j < BK; ++j)
-        for (int t = 0; t < L; ++t) idsrow[(size_t)j * ids_ld + t] = ids[(size_t)j * L + t];
-    GenState gs{};
-    gs.cur_len = L; gs.prompt_len = prompt_len; gs.max_length = gp->max_length; gs.min_new_tokens = gp->min_new_tokens;
-    gs.step = step; gs.has_last_scores = has_last_scores;
-    const SampleConfig sc = make_sample_config(gp, BK, use_cfg != 0, V, ids_ld);
-    std::vector<int> zeros(rows, 0);
-    std::vector<float> empty(BK, -1.0e9f);
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_ids.p, idsrow.data(), idsrow.size() * 8, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_vflags.p, vflags, c.vocab_size_in, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_state.p, &gs, sizeof(gs), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_cfg.p, &sc, sizeof(sc), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->g_leftpad.p, zeros.data(), rows * 4, cudaMemcpyHostToDevice, st));
+        for (int t = 0; t < ids_ld; ++t) idsrow[(size_t)j * ids_ld + t] = t < L ? ids[(size_t)j * L + t] : gp->pad_token_id;
+    std::memcpy(vf, vflags, c.vocab_size_in);
+    *gs = GenState{};
+    gs->cur_len = L; gs->prompt_len = prompt_len; gs->max_length = gp->max_length; gs->min_new_tokens = gp->min_new_tokens;
+    gs->step = step; gs->has_last_scores = has_last_scores;
+    *sc = make_sample_config(gp, BK, use_cfg != 0, V, ids_ld);
+    std::memcpy(runscore, run_scores, BK * sizeof(float));
+    for (int j = 0; j < BK; ++j) finscore[j] = -1.0e9f;      // an empty finished store
+    MB_TRY(sg.upload(m->g_ids.p, idsrow, (size_t)BK * ids_ld));
+    MB_TRY(sg.upload(m->g_vflags.p, vf, c.vocab_size_in));
+    MB_TRY(sg.upload(m->g_state.p, gs, 1));
+    MB_TRY(sg.upload(m->g_cfg.p, sc, 1));
+    MB_TRY(sg.upload(m->b_runscore.p, runscore, BK));
+    MB_TRY(sg.upload(m->b_finscore.p, finscore, BK));
+    MB_TRY(sg.end());
+    MB_CUDA_CHECK(cudaMemsetAsync(m->g_leftpad.p, 0, rows * sizeof(int), st));
     MB_CUDA_CHECK(cudaMemsetAsync(m->b_kvsrc.p, 0, (size_t)rows * ids_ld * sizeof(int), st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->b_runscore.p, run_scores, BK * 4, cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaMemcpyAsync(m->b_finscore.p, empty.data(), BK * 4, cudaMemcpyHostToDevice, st));
     MB_CUDA_CHECK(cudaMemsetAsync(m->b_finlen.p, 0, BK * sizeof(int), st));
     MB_CUDA_CHECK(cudaMemsetAsync(m->b_finflag.p, 0, BK, st));
     MB_CUDA_CHECK(cudaMemsetAsync(m->b_unsat.p, 1, B, st));
     MB_CUDA_CHECK(cudaMemcpyAsync(m->d_logits.p, logits, (size_t)rows * V * 4, cudaMemcpyDeviceToDevice, st));
-    MB_CUDA_CHECK(cudaStreamSynchronize(st));
-    MB_TRY(launch_prompt_scan(m->g_ids.as<long long>(), ids_ld, BK, L, m->g_vflags.as<unsigned char>(), sc.ts_start, sc.ts_end,
+    MB_TRY(launch_prompt_scan(m->g_ids.as<long long>(), ids_ld, BK, L, m->g_vflags.as<unsigned char>(), sc->ts_start, sc->ts_end,
                               m->g_lastts.as<int>(), st));
     BeamParams bp = beam_params(m, rows, K);
     bp.dbg_logprobs = logprobs_out;

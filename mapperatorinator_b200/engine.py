@@ -182,11 +182,27 @@ class ModelEngine:
         p, eos_ids, gk = self._generate_params(layout, generate_kwargs, position_rule)
         B, P = prompt.shape
         use_cfg = negative_prompt is not None and p.cfg_scale > 1.0
+        ids, msk, neg, nmsk, vflags, slots_a = self._prompt_args(slots, prompt, prompt_mask, negative_prompt if use_cfg else None, layout,
+                                                                 eos_ids)
+        out = np.zeros((B, p.max_length), dtype=np.int64)
+        out_len = C.c_int32(0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.mb200_model_generate(
+                self.handle, slots_a.ctypes.data, B, ids.ctypes.data, None if msk is None else msk.ctypes.data, P,
+                None if neg is None else neg.ctypes.data, None if nmsk is None else nmsk.ctypes.data, vflags.ctypes.data,
+                C.byref(p), out.ctypes.data, C.byref(out_len), _stream()))
+        L = out_len.value
+        return torch.from_numpy(out.reshape(-1)[: B * L].reshape(B, L).copy())
 
+    def _prompt_args(self, slots: Sequence[int], prompt: torch.Tensor, prompt_mask: Optional[torch.Tensor],
+                     negative_prompt: Optional[torch.Tensor], layout: TokenLayout, eos_ids: Sequence[int]):
+        """The arguments of `generate` and `generate_beams` in the form of the C ABI -> (ids, mask | None, negative rows | None, their
+        mask | None, vflags, slots).  `negative_prompt` is given only for a guided call."""
+        B = prompt.shape[0]
         ids = np.ascontiguousarray(prompt.detach().cpu().numpy().astype(np.int64))
         msk = None if prompt_mask is None else np.ascontiguousarray(prompt_mask.detach().cpu().numpy().astype(np.uint8))
         neg = nmsk = None
-        if use_cfg:
+        if negative_prompt is not None:
             neg_full = ids.copy()      # prepare_inputs_for_generation: ids.repeat(2); [:B, :neg_len] = negative prompt
             npn = negative_prompt.detach().cpu().numpy().astype(np.int64)
             neg_full[:, :npn.shape[1]] = npn
@@ -197,15 +213,7 @@ class ModelEngine:
         vflags = self._vflags.get(layout, eos_ids)
         slots_a = np.ascontiguousarray(np.asarray(list(slots), dtype=np.int32))
         assert slots_a.shape[0] == B
-        out = np.zeros((B, p.max_length), dtype=np.int64)
-        out_len = C.c_int32(0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.mb200_model_generate(
-                self.handle, slots_a.ctypes.data, B, ids.ctypes.data, None if msk is None else msk.ctypes.data, P,
-                None if neg is None else neg.ctypes.data, None if nmsk is None else nmsk.ctypes.data, vflags.ctypes.data,
-                C.byref(p), out.ctypes.data, C.byref(out_len), _stream()))
-        L = out_len.value
-        return torch.from_numpy(out.reshape(-1)[: B * L].reshape(B, L).copy())
+        return ids, msk, neg, nmsk, vflags, slots_a
 
     def _ragged_args(self, requests: Sequence[tuple], layout: TokenLayout):
         """Validates independent batch-1 requests `(slot, prompt ids (P_r,) without padding, generate_kwargs, negative prompt | None)` on
@@ -296,18 +304,8 @@ class ModelEngine:
         if rows > self.max_batch:
             raise ValueError(f"beam search needs batch * num_beams{' * 2 (classifier-free guidance)' if use_cfg else ''} = {rows} "
                              f"decoder rows; this engine was built with max_batch={self.max_batch}")
-        ids = np.ascontiguousarray(prompt.detach().cpu().numpy().astype(np.int64))
-        msk = None if prompt_mask is None else np.ascontiguousarray(prompt_mask.detach().cpu().numpy().astype(np.uint8))
-        neg = nmsk = None
-        if use_cfg:
-            neg_full = ids.copy()
-            npn = negative_prompt.detach().cpu().numpy().astype(np.int64)
-            neg_full[:, :npn.shape[1]] = npn
-            neg = np.ascontiguousarray(neg_full)
-            nmsk = np.ascontiguousarray(msk.copy() if msk is not None else np.ones_like(ids, dtype=np.uint8))
-        vflags = self._vflags.get(layout, eos_ids)
-        slots_a = np.ascontiguousarray(np.asarray(list(slots), dtype=np.int32))
-        assert slots_a.shape[0] == B
+        ids, msk, neg, nmsk, vflags, slots_a = self._prompt_args(slots, prompt, prompt_mask, negative_prompt if use_cfg else None, layout,
+                                                                 eos_ids)
         fill = p.pad_token_id if p.pad_token_id else eos_ids[0]          # HF: `pad_token_id or eos_token_id[0]`
         out = np.zeros((B, p.max_length), dtype=np.int64)
         scores = np.zeros(B, dtype=np.float32)
@@ -366,10 +364,8 @@ class ModelEngine:
 
     def forward_logits(self, slots: Sequence[int], ids: torch.Tensor, mask: Optional[torch.Tensor],
                        position_rule: str = "arange") -> torch.Tensor:
-        B, L = ids.shape
-        a = np.ascontiguousarray(ids.detach().cpu().numpy().astype(np.int64))
-        m = None if mask is None else np.ascontiguousarray(mask.detach().cpu().numpy().astype(np.uint8))
-        slots_a = np.ascontiguousarray(np.asarray(list(slots), dtype=np.int32))
+        a, m, slots_a = self._score_args(slots, ids, mask)
+        B, L = a.shape
         out = torch.empty(B, L, self.cfg.vocab_size_out, device=self.device, dtype=torch.float32)
         with torch.cuda.device(self.device):
             _lib.check(self.lib.mb200_model_forward_logits(self.handle, slots_a.ctypes.data, B, a.ctypes.data,
@@ -378,7 +374,8 @@ class ModelEngine:
         return out
 
     def _score_args(self, slots: Sequence[int], ids: torch.Tensor, mask: Optional[torch.Tensor]):
-        """Validates a scoring call on the host (ValueError before anything is launched) -> (ids, mask, slots) as numpy arrays."""
+        """Validates a teacher-forced call (`forward_logits`, `score_tokens`) on the host (ValueError before anything is launched)
+        -> (ids, mask, slots) as numpy arrays."""
         if ids.dim() != 2:
             raise ValueError(f"ids must be [B, L], got shape {tuple(ids.shape)}")
         B, L = ids.shape

@@ -151,6 +151,26 @@ def test_rejections(tiny):
     for bad in (cfg.vocab_size_in, -1):
         with pytest.raises(ValueError, match="token ids"):
             model_score(model, _mk(cfg, torch.tensor([[3700, bad, 1]]), None, 1), {})
+    # an encoder slot outside the resident ones, or one slot per row missing, is refused before anything is launched: by the Python
+    # wrapper, and by the engine itself for a caller of the C ABI
+    from mapperatorinator_b200 import _lib
+    eng, lib = model.engine, _lib.load()
+    before = lib.mb200_launch_count()
+    with pytest.raises(ValueError, match="encoder slots"):
+        eng.forward_logits([eng.max_windows], ids, None)
+    with pytest.raises(ValueError, match="encoder slots"):
+        eng.forward_logits([0, 1], ids, None)
+    B, L = ids.shape
+    a = np.ascontiguousarray(ids.numpy().astype(np.int64))
+    slots = np.array([eng.max_windows], dtype=np.int32)
+    logits = torch.empty(B, L, cfg.vocab_size_out, device="cuda")
+    assert lib.mb200_model_forward_logits(eng.handle, slots.ctypes.data, B, a.ctypes.data, None, L, 0, logits.data_ptr(), None) != 0
+    assert b"encoder slot out of range" in lib.mb200_last_error()
+    stats = [torch.empty(B, L, device="cuda") for _ in range(3)] + [torch.empty(B, L, device="cuda", dtype=torch.int64)]
+    assert lib.mb200_model_score_tokens(eng.handle, slots.ctypes.data, B, a.ctypes.data, None, L, 0, *(t.data_ptr() for t in stats),
+                                        None) != 0
+    assert b"encoder slot out of range" in lib.mb200_last_error()
+    assert lib.mb200_launch_count() == before
 
 
 def test_generate_after_score_matches_fixture(tiny, layout):

@@ -245,6 +245,17 @@ def test_rejections_launch_nothing_and_leave_stream_and_engine_usable(tiny16, la
             eng.score_tokens([1], q["prompt"], None)
         with pytest.raises(RuntimeError, match="already open"):
             eng.open_stream(layout, 1)
+        # the PDL toggle would destroy the stream's step graph; the parity hooks and the step profiler write its state
+        with pytest.raises(RuntimeError, match="decode stream is open"):
+            eng.set_option("pdl", 1)
+        ids, V = q["prompt"], cfg.vocab_size_out
+        with pytest.raises(RuntimeError, match="decode stream is open"):
+            eng.logits_chain(torch.zeros(1, V, device="cuda"), ids, ids.shape[1], layout, dict(q["gk"]))
+        with pytest.raises(RuntimeError, match="decode stream is open"):
+            eng.beam_step(torch.zeros(2, V, device="cuda"), ids.repeat(2, 1), torch.zeros(2), 2, ids.shape[1], layout, dict(q["gk"]))
+        out_us = np.zeros(4, dtype=np.float32)
+        with pytest.raises(RuntimeError, match="decode stream is open"):
+            _lib.check(lib.mb200_model_profile_step(eng.handle, 1, 1, 64, 1, out_us.ctypes.data, None))
         assert lib.mb200_launch_count() == before
         got = {}
         _drain(stream, got, {row: 0})
