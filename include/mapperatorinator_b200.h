@@ -61,8 +61,17 @@ void mb200_model_destroy(mb200_model* m);
 /* Upload one tensor by its reference state_dict() name (SURVEY Appendix A.7); data is HOST float32. Unknown names that
  * the inference path does not read (loss_fn.weight, decoder.embed_tokens.weight, spectrogram.*) are accepted and ignored. */
 int mb200_model_set_weight(mb200_model* m, const char* name, const float* data, int64_t numel);
-/* Checks that every required tensor was set and packs fused weights (q|k|v stacking, conv tap-major layout). */
+/* The same for a tensor held in bf16 (a model loaded at bf16 precision): bits are HOST bf16 bit patterns. The engine keeps the
+ * widened (exact) fp32 values and remembers that the tensor arrived as bf16. */
+int mb200_model_set_weight_bf16(mb200_model* m, const char* name, const uint16_t* bits, int64_t numel);
+/* Checks that every required tensor was set and packs fused weights (q|k|v stacking, conv tap-major layout).
+ * When every matrix the token loop streams arrived as bf16 (q|k|v, out, cross q, cross out, fc1 and fc2 of every decoder layer, and
+ * proj_out), every packed element is still a bf16 value and every row length is a multiple of 8, the engine also keeps a bf16 copy of
+ * those matrices, which every token-loop driver streams (half the bytes, the same result bits); the prefill, the cross K/V projection
+ * and the teacher-forced passes read the fp32 weights. */
 int mb200_model_finalize(mb200_model* m);
+/* 2 when the engine holds the bf16 token-loop store, else 4. After finalize. */
+int mb200_model_token_weight_bytes(const mb200_model* m, int32_t* bytes);
 
 /* OsuTEncoder.forward (modeling_mapperatorinator.py:392-443) + the cross-attention K/V projection of every decoder
  * layer (HF modeling_whisper.py:331-338), for `n_windows` windows of raw PCM, written to slots
@@ -236,6 +245,8 @@ int mb200_dit_apply_sliders(mb200_dit* d, float* x, int32_t N, int32_t T, void* 
  * ------------------------------------------------------------------------------------------------------------------ */
 /* Number of engine kernels launched by this process so far (graph replays count every node). */
 int64_t mb200_launch_count(void);
+/* The launches among those whose weights are a bf16 token-loop store (bf16 GEMVs and bf16 megakernels). */
+int64_t mb200_wbf16_launch_count(void);
 /* option "pdl": 1 = capture the token-step graph with programmatic dependent launch edges. */
 int mb200_model_set_option(mb200_model* m, const char* name, int32_t value);
 /* Parity hook for the fused logits-processor chain (server.py:106-134 + HF min-new-tokens / top-k / top-p + selection): ONE selection
@@ -329,6 +340,12 @@ int mb200_op_gemv(const float* x, int64_t x_ld, int32_t B, int32_t K, int32_t xm
                   const float* W, int64_t ldw, int32_t N, const float* bias, const float* R, int64_t r_ld, const mb200_gemv_seg* segs,
                   int32_t nseg, int32_t cur_len, const int32_t* ragged_cur_len, const int32_t* ragged_finished, int32_t n_req,
                   int32_t form, void* cuda_stream);
+/* mb200_op_gemv with W given as bf16 bits (DEVICE uint16 [N rows of K at stride ldw]), through the bf16 GEMV the token loop runs on a
+ * bf16 store. K and ldw must be multiples of 8 and W 16-byte aligned. */
+int mb200_op_gemv_bf16(const float* x, int64_t x_ld, int32_t B, int32_t K, int32_t xmode, const float* ln_w, const float* ln_b, float eps,
+                       const uint16_t* W, int64_t ldw, int32_t N, const float* bias, const float* R, int64_t r_ld, const mb200_gemv_seg* segs,
+                       int32_t nseg, int32_t cur_len, const int32_t* ragged_cur_len, const int32_t* ragged_finished, int32_t n_req,
+                       int32_t form, void* cuda_stream);
 /* Tuning / tests: tensor-core (wgmma, 3xTF32) flash attention on or off, and the minimum number of queries for which it is used
    (attention_tc.cu; replaces the SIMT kernel for the encoder self-attention of HF modeling_whisper.py:286-358 and the DiT band of
    osu_diffusion/utils/models.py:145-151). */

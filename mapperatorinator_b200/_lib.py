@@ -54,15 +54,16 @@ class DitMaskC(C.Structure):
 ABI_SYMBOLS = [
     "mb200_abi_version", "mb200_last_error",
     "mb200_mel_create", "mb200_mel_destroy", "mb200_mel_forward",
-    "mb200_model_create", "mb200_model_destroy", "mb200_model_set_weight", "mb200_model_finalize", "mb200_model_encode",
+    "mb200_model_create", "mb200_model_destroy", "mb200_model_set_weight", "mb200_model_set_weight_bf16", "mb200_model_finalize",
+    "mb200_model_token_weight_bytes", "mb200_model_encode",
     "mb200_model_generate", "mb200_model_generate_beams", "mb200_model_generate_ragged", "mb200_model_forward_logits",
     "mb200_stream_open", "mb200_stream_admit", "mb200_stream_run", "mb200_stream_take", "mb200_stream_close",
     "mb200_model_score_tokens",
     "mb200_dit_create", "mb200_dit_destroy", "mb200_dit_set_weight", "mb200_dit_finalize", "mb200_dit_forward_with_cfg",
     "mb200_dit_sample_loop", "mb200_dit_set_option", "mb200_dit_set_sliders", "mb200_dit_apply_sliders",
-    "mb200_launch_count", "mb200_model_set_option", "mb200_model_profile_step", "mb200_model_read_trace", "mb200_model_mega_stats", "mb200_model_logits_chain",
+    "mb200_launch_count", "mb200_wbf16_launch_count", "mb200_model_set_option", "mb200_model_profile_step", "mb200_model_read_trace", "mb200_model_mega_stats", "mb200_model_logits_chain",
     "mb200_model_beam_step",
-    "mb200_op_gemm", "mb200_op_gemm_tc", "mb200_set_tensor_cores", "mb200_op_layernorm", "mb200_op_attention", "mb200_op_decode_attention", "mb200_op_gemv", "mb200_set_attention_tc", "mb200_audio_out_frames", "mb200_audio_ingest",
+    "mb200_op_gemm", "mb200_op_gemm_tc", "mb200_set_tensor_cores", "mb200_op_layernorm", "mb200_op_attention", "mb200_op_decode_attention", "mb200_op_gemv", "mb200_op_gemv_bf16", "mb200_set_attention_tc", "mb200_audio_out_frames", "mb200_audio_ingest",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -86,7 +87,9 @@ def load() -> C.CDLL:
     lib.mb200_model_create.argtypes = [C.POINTER(vp), C.POINTER(ModelConfigC), vp]
     lib.mb200_model_destroy.argtypes = [vp]; lib.mb200_model_destroy.restype = None
     lib.mb200_model_set_weight.argtypes = [vp, C.c_char_p, vp, i64]
+    lib.mb200_model_set_weight_bf16.argtypes = [vp, C.c_char_p, vp, i64]
     lib.mb200_model_finalize.argtypes = [vp]
+    lib.mb200_model_token_weight_bytes.argtypes = [vp, C.POINTER(i32)]
     lib.mb200_model_encode.argtypes = [vp, vp, i32, i32, vp, vp]
     lib.mb200_model_generate.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp, vp, C.POINTER(GenerateParamsC), vp, C.POINTER(i32), vp]
     lib.mb200_model_generate_beams.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp, vp, C.POINTER(GenerateParamsC), i32, i64, vp,
@@ -101,6 +104,7 @@ def load() -> C.CDLL:
     lib.mb200_model_score_tokens.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, vp, vp, vp, vp]
     lib.mb200_model_set_option.argtypes = [vp, C.c_char_p, i32]
     lib.mb200_launch_count.restype = i64
+    lib.mb200_wbf16_launch_count.restype = i64
     lib.mb200_model_profile_step.argtypes = [vp, i32, i32, i32, i32, vp, vp]
     lib.mb200_model_read_trace.argtypes = [vp, vp, i32]
     lib.mb200_model_mega_stats.argtypes = [vp, vp, i32]
@@ -125,6 +129,7 @@ def load() -> C.CDLL:
     lib.mb200_op_decode_attention.argtypes = [vp, vp, i32, i32, i32, i32, vp, i32, i32, vp, i64, i32, i32, vp, i64, vp, vp, i32, vp, vp]
     lib.mb200_op_gemv.argtypes = [vp, i64, i32, i32, i32, vp, vp, f32, vp, i64, i32, vp, vp, i64, C.POINTER(GemvSegC), i32, i32, vp, vp,
                                   i32, i32, vp]
+    lib.mb200_op_gemv_bf16.argtypes = lib.mb200_op_gemv.argtypes
     lib.mb200_audio_out_frames.argtypes = [i64, i32, i32]
     lib.mb200_audio_out_frames.restype = i64
     lib.mb200_audio_ingest.argtypes = [vp, i64, i32, i32, i32, i32, vp, vp, vp]

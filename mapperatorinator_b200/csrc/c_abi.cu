@@ -11,6 +11,7 @@ namespace mb200 {
 static thread_local std::string g_last_error;
 void set_last_error(const std::string& msg) { g_last_error = msg; }
 long long g_launch_count = 0;
+long long g_wbf16_launch_count = 0;
 StepProfiler g_prof;
 }  // namespace mb200
 
@@ -23,6 +24,7 @@ struct mb200_mel {
 
 extern "C" int mb200_abi_version(void) { return MB200_ABI_VERSION; }
 extern "C" int64_t mb200_launch_count(void) { return (int64_t)g_launch_count; }
+extern "C" int64_t mb200_wbf16_launch_count(void) { return (int64_t)g_wbf16_launch_count; }
 extern "C" const char* mb200_last_error(void) { return g_last_error.c_str(); }
 
 extern "C" int mb200_mel_create(mb200_mel** out, const mb200_mel_config* cfg, const float* mel_basis) {
@@ -191,14 +193,16 @@ extern "C" int mb200_op_decode_attention(const float* q, const float* kv, int32_
 }
 
 // One GEMV phase through launch_gemv, with the GemvParams a token step builds and the call state (GenState, RowStates) owned here.
-extern "C" int mb200_op_gemv(const float* x, int64_t x_ld, int32_t B, int32_t K, int32_t xmode, const float* ln_w, const float* ln_b,
-                             float eps, const float* W, int64_t ldw, int32_t N, const float* bias, const float* R, int64_t r_ld,
-                             const mb200_gemv_seg* segs, int32_t nseg, int32_t cur_len, const int32_t* ragged_cur_len,
-                             const int32_t* ragged_finished, int32_t n_req, int32_t form, void* stream) {
+// w_bf16: W holds bf16 bits (the token loop's bf16 store).
+static int op_gemv(const float* x, int64_t x_ld, int32_t B, int32_t K, int32_t xmode, const float* ln_w, const float* ln_b, float eps,
+                   const void* W, bool w_bf16, int64_t ldw, int32_t N, const float* bias, const float* R, int64_t r_ld,
+                   const mb200_gemv_seg* segs, int32_t nseg, int32_t cur_len, const int32_t* ragged_cur_len,
+                   const int32_t* ragged_finished, int32_t n_req, int32_t form, void* stream) {
     MB_REQUIRE(x && W && segs, "null argument");
     MB_REQUIRE(B >= 1 && N >= 1 && K >= 4, "need B >= 1, N >= 1, K >= 4");
     MB_REQUIRE(x_ld >= K && ldw >= K && (!R || r_ld >= N), "a row stride is shorter than its row");
     MB_REQUIRE(reinterpret_cast<uintptr_t>(x) % 16 == 0 && reinterpret_cast<uintptr_t>(W) % 16 == 0, "x and W are read as float4");
+    MB_REQUIRE(!w_bf16 || (K % 8 == 0 && ldw % 8 == 0), "bf16 weights are read 4 at a time from 16-byte rows: K and ldw must be multiples of 8");
     MB_REQUIRE(xmode == X_PLAIN || xmode == X_LAYERNORM, "unknown input mode");
     MB_REQUIRE(xmode != X_LAYERNORM || (ln_w && ln_b), "a LayerNorm input needs its weight and bias");
     MB_REQUIRE(nseg >= 1 && nseg <= 3, "1 to 3 output segments");
@@ -207,7 +211,7 @@ extern "C" int mb200_op_gemv(const float* x, int64_t x_ld, int32_t B, int32_t K,
     bool positional = false;
     GemvParams g{};
     g.xmode = xmode; g.x = x; g.x_ld = x_ld; g.ln_w = ln_w; g.ln_b = ln_b; g.eps = eps;
-    g.W = W; g.ldw = ldw; g.bias = bias; g.K = K; g.N = N; g.B = B; g.R = R; g.r_ld = r_ld;
+    g.W = reinterpret_cast<const float*>(W); g.ldw = ldw; g.bias = bias; g.K = K; g.N = N; g.B = B; g.R = R; g.r_ld = r_ld;
     g.nseg = nseg;
     for (int i = 0; i < nseg; ++i) {
         const mb200_gemv_seg& s = segs[i];
@@ -239,9 +243,25 @@ extern "C" int mb200_op_gemv(const float* x, int64_t x_ld, int32_t B, int32_t K,
     MB_CUDA_CHECK(cudaMemcpyAsync(op_state.p, &gs, sizeof(GenState), cudaMemcpyHostToDevice, st));
     if (ragged) MB_CUDA_CHECK(cudaMemcpyAsync(reinterpret_cast<GenState*>(op_state.p) + 1, rs.data(), rs.size() * sizeof(RowState), cudaMemcpyHostToDevice, st));
     g.st = reinterpret_cast<const GenState*>(op_state.p);
-    const int rc = launch_gemv(g, st, false, ragged, form);     // also where the shape requirements of the kernels are checked
+    const int rc = launch_gemv(g, st, false, ragged, form, w_bf16);     // also where the shape requirements of the kernels are checked
     MB_CUDA_CHECK(cudaStreamSynchronize(st));      // the host-side state above goes out of scope
     return rc;
+}
+
+extern "C" int mb200_op_gemv(const float* x, int64_t x_ld, int32_t B, int32_t K, int32_t xmode, const float* ln_w, const float* ln_b,
+                             float eps, const float* W, int64_t ldw, int32_t N, const float* bias, const float* R, int64_t r_ld,
+                             const mb200_gemv_seg* segs, int32_t nseg, int32_t cur_len, const int32_t* ragged_cur_len,
+                             const int32_t* ragged_finished, int32_t n_req, int32_t form, void* stream) {
+    return op_gemv(x, x_ld, B, K, xmode, ln_w, ln_b, eps, W, false, ldw, N, bias, R, r_ld, segs, nseg, cur_len, ragged_cur_len, ragged_finished,
+                   n_req, form, stream);
+}
+
+extern "C" int mb200_op_gemv_bf16(const float* x, int64_t x_ld, int32_t B, int32_t K, int32_t xmode, const float* ln_w, const float* ln_b,
+                                  float eps, const uint16_t* W, int64_t ldw, int32_t N, const float* bias, const float* R, int64_t r_ld,
+                                  const mb200_gemv_seg* segs, int32_t nseg, int32_t cur_len, const int32_t* ragged_cur_len,
+                                  const int32_t* ragged_finished, int32_t n_req, int32_t form, void* stream) {
+    return op_gemv(x, x_ld, B, K, xmode, ln_w, ln_b, eps, W, true, ldw, N, bias, R, r_ld, segs, nseg, cur_len, ragged_cur_len, ragged_finished,
+                   n_req, form, stream);
 }
 
 // tuning / tests: minimum query count for the tensor-core attention path (0 disables it)

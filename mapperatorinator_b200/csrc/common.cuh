@@ -33,6 +33,7 @@ void set_last_error(const std::string& msg);
 
 // ---- measurement hooks: every launch_* bumps the counter; the step profiler brackets decode-path launches with events ----
 extern long long g_launch_count;
+extern long long g_wbf16_launch_count;      // the launches among them whose weights are a bf16 store (GEMV and megakernel)
 struct StepProfiler {
     bool on = false;
     cudaEvent_t ev[1024];
@@ -46,9 +47,11 @@ extern StepProfiler g_prof;
 struct CapturedGraph {
     cudaGraphExec_t exec = nullptr;
     long long nodes = 0;          // launches the body counted while it was captured
+    long long wbf16_nodes = 0;    // ... of which read a bf16 weight store
     int launch(cudaStream_t st, int times = 1) {
         for (int i = 0; i < times; ++i) MB_CUDA_CHECK(cudaGraphLaunch(exec, st));
         g_launch_count += (long long)times * nodes;
+        g_wbf16_launch_count += (long long)times * wbf16_nodes;
         return 0;
     }
 };
@@ -61,11 +64,13 @@ int capture_graph(cudaStream_t& cap_stream, cudaStream_t st, Body&& body, Captur
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
     cudaGraph_t graph;
     MB_CUDA_CHECK(cudaStreamBeginCapture(cap_stream, cudaStreamCaptureModeThreadLocal));
-    const long long before = g_launch_count;
+    const long long before = g_launch_count, before16 = g_wbf16_launch_count;
     const int rc = body(cap_stream);
     const cudaError_t e = cudaStreamEndCapture(cap_stream, &graph);
     out->nodes = g_launch_count - before;
+    out->wbf16_nodes = g_wbf16_launch_count - before16;
     g_launch_count = before;
+    g_wbf16_launch_count = before16;
     if (rc) {
         if (e == cudaSuccess) cudaGraphDestroy(graph);
         return rc;

@@ -20,7 +20,8 @@ namespace {
 
 constexpr int GEMV_THREADS = 128, GEMV_WARPS = GEMV_THREADS / 32;
 
-template <int NB, bool RAGGED = false>
+// WBF16: p.W holds bf16 bits, row n at element n * p.ldw (decode_device.cuh gemv_dot)
+template <int NB, bool RAGGED = false, bool WBF16 = false>
 __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(GemvParams p) {
     extern __shared__ __align__(16) float xs[];   // [NB][K] activations, then 32 floats of LayerNorm reduction scratch
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -31,7 +32,7 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(GemvParams p) {
         gemv_stage_x<NB, GEMV_THREADS>(p, b0, xs, xs + NB * p.K, tid);
         __syncthreads();
         for (int n = blockIdx.x * GEMV_WARPS + warp; n < p.N; n += gridDim.x * GEMV_WARPS)
-            gemv_row<NB, true, RAGGED>(p, n, p.W + (long long)n * p.ldw, xs, b0, lane, cur_pos);
+            gemv_row<NB, true, RAGGED, WBF16>(p, n, gemv_wrow<WBF16>(p.W, (long long)n * p.ldw), xs, b0, lane, cur_pos);
         __syncthreads();
     }
 }
@@ -42,7 +43,8 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(GemvParams p) {
 // the two forms to the same bits.
 constexpr int MEGA_GEMV_THREADS = SAMPLE_THREADS;      // decode_mega.cu's MEGA_THREADS
 
-template <int NB>
+// WBF16: the rows are bf16 bits (K a multiple of 8), copied to shared memory as they are: half the bytes of the fp32 slice.
+template <int NB, bool WBF16 = false>
 __global__ void __launch_bounds__(MEGA_GEMV_THREADS) gemv_mega_body_kernel(GemvParams p) {
     extern __shared__ __align__(16) float sm[];   // [rpc][K] weight rows, [NB][K] activations, 32 floats of LayerNorm reduction scratch
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -50,18 +52,18 @@ __global__ void __launch_bounds__(MEGA_GEMV_THREADS) gemv_mega_body_kernel(GemvP
     pdl_wait();
     const int rpc = (p.N + (int)gridDim.x - 1) / (int)gridDim.x;
     const int r0 = min(p.N, (int)blockIdx.x * rpc), r1 = min(p.N, r0 + rpc);
-    const int K4 = p.K >> 2;
+    const int KV = WBF16 ? p.K >> 3 : p.K >> 2;     // 16-byte vectors per weight row
     float* wbuf = sm;
-    float* xs = sm + (long long)rpc * p.K;
-    for (int e = tid; e < (r1 - r0) * K4; e += MEGA_GEMV_THREADS) {
-        const int r = e / K4, c = e - r * K4;
-        reinterpret_cast<float4*>(wbuf)[e] = __ldg(reinterpret_cast<const float4*>(p.W + (long long)(r0 + r) * p.ldw) + c);
+    float* xs = sm + (WBF16 ? (long long)rpc * (p.K >> 1) : (long long)rpc * p.K);
+    for (int e = tid; e < (r1 - r0) * KV; e += MEGA_GEMV_THREADS) {
+        const int r = e / KV, c = e - r * KV;
+        reinterpret_cast<float4*>(wbuf)[e] = __ldg(reinterpret_cast<const float4*>(gemv_wrow<WBF16>(p.W, (long long)(r0 + r) * p.ldw)) + c);
     }
     gemv_stage_x<NB, MEGA_GEMV_THREADS>(p, 0, xs, xs + NB * p.K, tid);
     __syncthreads();
     const int cur_pos = p.st ? p.st->cur_len - 1 : 0;
     for (int n = r0 + warp; n < r1; n += MEGA_GEMV_THREADS / 32)
-        gemv_row<NB, false>(p, n, wbuf + (long long)(n - r0) * p.K, xs, 0, lane, cur_pos);
+        gemv_row<NB, false, false, WBF16>(p, n, gemv_wrow<WBF16>(wbuf, (long long)(n - r0) * p.K), xs, 0, lane, cur_pos);
 }
 
 template <int KMAX, bool TABLE = false>
@@ -203,42 +205,38 @@ int launch_with_attrs(Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_
 
 }  // namespace
 
-int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged, int form) {
-    MB_REQUIRE(p.K % 4 == 0 && p.ldw % 4 == 0 && p.x_ld % 4 == 0, "GEMV K / ldw / x_ld must be multiples of 4");
-    MB_REQUIRE(p.xmode != X_LAYERNORM || p.K <= 1024, "fused LayerNorm prologue supports K <= 1024");
-    MB_REQUIRE(form == GEMV_FORM_KERNEL || form == GEMV_FORM_MEGA, "unknown GEMV form");
-    MB_REQUIRE(form != GEMV_FORM_MEGA || (!ragged && p.B <= 2), "the megakernel's GEMV body runs 1 or 2 rows, not ragged");
-    if (p.B <= 0 || p.N <= 0) return 0;
+template <bool WBF16>
+static int launch_gemv_impl(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged, int form) {
     if (form == GEMV_FORM_MEGA) {
         // a 132-CTA grid like the megakernel's on an H100, more CTAs when that many rows per CTA would not fit shared memory
-        const size_t limit = 200 * 1024, fixed = ((size_t)p.B * p.K + 32) * sizeof(float), row = (size_t)p.K * sizeof(float);
+        const size_t limit = 200 * 1024, fixed = ((size_t)p.B * p.K + 32) * sizeof(float), row = (size_t)p.K * (WBF16 ? 2 : sizeof(float));
         MB_REQUIRE(fixed + row <= limit, "GEMV activation tile does not fit shared memory");
         const int rpc = (int)std::min<size_t>((p.N + 131) / 132, (limit - fixed) / row);
         static bool mega_configured = false;
         if (!mega_configured) {
-            MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_mega_body_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit));
-            MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_mega_body_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit));
+            MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_mega_body_kernel<1, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit));
+            MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_mega_body_kernel<2, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit));
             mega_configured = true;
         }
         const dim3 grid((p.N + rpc - 1) / rpc);       // the kernel's ceil(N / grid) is at most rpc
         const size_t smem = fixed + rpc * row;
         g_prof_class = 0;
-        return p.B == 1 ? launch_with_attrs(gemv_mega_body_kernel<1>, grid, dim3(MEGA_GEMV_THREADS), smem, stream, pdl, p)
-                        : launch_with_attrs(gemv_mega_body_kernel<2>, grid, dim3(MEGA_GEMV_THREADS), smem, stream, pdl, p);
+        return p.B == 1 ? launch_with_attrs(gemv_mega_body_kernel<1, WBF16>, grid, dim3(MEGA_GEMV_THREADS), smem, stream, pdl, p)
+                        : launch_with_attrs(gemv_mega_body_kernel<2, WBF16>, grid, dim3(MEGA_GEMV_THREADS), smem, stream, pdl, p);
     }
     int nb = p.B >= 8 ? 8 : (p.B > 4 ? 8 : (p.B > 2 ? 4 : p.B));
     const size_t smem = ((size_t)nb * p.K + 32) * sizeof(float);
     const int blocks = (p.N + GEMV_WARPS - 1) / GEMV_WARPS;
     static bool configured = false;
     if (!configured) {
-        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<1, false, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<2, false, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<4, false, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<8, false, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<1, true, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<2, true, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<4, true, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(gemv_kernel<8, true, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         configured = true;
     }
     MB_REQUIRE(smem <= 200 * 1024, "GEMV activation tile does not fit shared memory");
@@ -246,18 +244,32 @@ int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged,
     if (ragged) {
         MB_REQUIRE(p.st, "ragged GEMV needs the ragged state");
         switch (nb) {
-            case 1: return launch_with_attrs(gemv_kernel<1, true>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
-            case 2: return launch_with_attrs(gemv_kernel<2, true>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
-            case 4: return launch_with_attrs(gemv_kernel<4, true>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
-            default: return launch_with_attrs(gemv_kernel<8, true>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
+            case 1: return launch_with_attrs(gemv_kernel<1, true, WBF16>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
+            case 2: return launch_with_attrs(gemv_kernel<2, true, WBF16>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
+            case 4: return launch_with_attrs(gemv_kernel<4, true, WBF16>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
+            default: return launch_with_attrs(gemv_kernel<8, true, WBF16>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
         }
     }
     switch (nb) {
-        case 1: return launch_with_attrs(gemv_kernel<1>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
-        case 2: return launch_with_attrs(gemv_kernel<2>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
-        case 4: return launch_with_attrs(gemv_kernel<4>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
-        default: return launch_with_attrs(gemv_kernel<8>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
+        case 1: return launch_with_attrs(gemv_kernel<1, false, WBF16>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
+        case 2: return launch_with_attrs(gemv_kernel<2, false, WBF16>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
+        case 4: return launch_with_attrs(gemv_kernel<4, false, WBF16>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
+        default: return launch_with_attrs(gemv_kernel<8, false, WBF16>, dim3(blocks), dim3(GEMV_THREADS), smem, stream, pdl, p);
     }
+}
+
+int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged, int form, bool w_bf16) {
+    MB_REQUIRE(p.K % 4 == 0 && p.ldw % 4 == 0 && p.x_ld % 4 == 0, "GEMV K / ldw / x_ld must be multiples of 4");
+    MB_REQUIRE(!w_bf16 || (p.K % 8 == 0 && p.ldw % 8 == 0 && reinterpret_cast<uintptr_t>(p.W) % 16 == 0),
+               "bf16 GEMV weights need K and ldw multiples of 8 and 16-byte aligned rows");
+    MB_REQUIRE(p.xmode != X_LAYERNORM || p.K <= 1024, "fused LayerNorm prologue supports K <= 1024");
+    MB_REQUIRE(form == GEMV_FORM_KERNEL || form == GEMV_FORM_MEGA, "unknown GEMV form");
+    MB_REQUIRE(form != GEMV_FORM_MEGA || (!ragged && p.B <= 2), "the megakernel's GEMV body runs 1 or 2 rows, not ragged");
+    if (p.B <= 0 || p.N <= 0) return 0;
+    if (!w_bf16) return launch_gemv_impl<false>(p, stream, pdl, ragged, form);
+    const int rc = launch_gemv_impl<true>(p, stream, pdl, ragged, form);
+    if (rc == 0) ++g_wbf16_launch_count;
+    return rc;
 }
 
 int launch_decode_attention(const DecAttnParams& p, cudaStream_t stream, bool pdl, int form) {

@@ -188,21 +188,39 @@ __device__ __forceinline__ void gemv_row_operands(const GemvParams& p, int n, in
 // dot(W[n, :], xs[b, :]) for NB batch rows; lane b < NB ends up holding row b's sum in `mine`.  Four independent accumulation chains
 // per batch row (the x / y / z / w components of the float4 stream), merged as (x + y) + (z + w) before the shuffle tree.  Shared by
 // every decode driver (per-kernel GEMV, barrier megakernel, dataflow megakernel): same order, same bits.
-template <int NB, bool W_GLOBAL>
+// WBF16: the row holds bf16 bits (wrow_f is reinterpreted).  A lane loads the 4 weights of group idx as 8 bytes instead of 16, widens
+// them (exact) and runs the same FMAs in the same order, so the result is the bits of the fp32 kernel on the widened row.
+__device__ __forceinline__ float4 bf16x4_to_float4(uint2 v) {
+    return make_float4(__uint_as_float(v.x << 16), __uint_as_float(v.x & 0xffff0000u), __uint_as_float(v.y << 16), __uint_as_float(v.y & 0xffff0000u));
+}
+template <int NB, bool W_GLOBAL, bool WBF16 = false>
 __device__ __forceinline__ float gemv_dot(int K, const float* wrow_f, const float* xs, int lane, unsigned long long* dbg = nullptr) {
     const int K4 = K >> 2;
-    const float4* wrow = reinterpret_cast<const float4*>(wrow_f);
     float4 acc[NB];
 #pragma unroll
     for (int b = 0; b < NB; ++b) acc[b] = make_float4(0.f, 0.f, 0.f, 0.f);
-    constexpr int U = W_GLOBAL ? 12 : 6;     // float4 loads in flight per lane (same j-major summation order either way)
+    constexpr int U = W_GLOBAL ? 12 : 6;     // loads in flight per lane (same j-major summation order either way)
     for (int base = 0; base < K4; base += 32 * U) {
         float4 w[U];
+        if constexpr (WBF16) {
+            const uint2* wrow = reinterpret_cast<const uint2*>(wrow_f);
+            uint2 raw[U];
 #pragma unroll
-        for (int j = 0; j < U; ++j) {
-            int idx = base + j * 32 + lane;
-            if (W_GLOBAL) w[j] = idx < K4 ? __ldg(wrow + idx) : make_float4(0, 0, 0, 0);
-            else          w[j] = idx < K4 ? wrow[idx] : make_float4(0, 0, 0, 0);
+            for (int j = 0; j < U; ++j) {
+                int idx = base + j * 32 + lane;
+                if (W_GLOBAL) raw[j] = idx < K4 ? __ldg(wrow + idx) : make_uint2(0, 0);
+                else          raw[j] = idx < K4 ? wrow[idx] : make_uint2(0, 0);
+            }
+#pragma unroll
+            for (int j = 0; j < U; ++j) w[j] = bf16x4_to_float4(raw[j]);
+        } else {
+            const float4* wrow = reinterpret_cast<const float4*>(wrow_f);
+#pragma unroll
+            for (int j = 0; j < U; ++j) {
+                int idx = base + j * 32 + lane;
+                if (W_GLOBAL) w[j] = idx < K4 ? __ldg(wrow + idx) : make_float4(0, 0, 0, 0);
+                else          w[j] = idx < K4 ? wrow[idx] : make_float4(0, 0, 0, 0);
+            }
         }
 #pragma unroll
         for (int j = 0; j < U; ++j) {
@@ -227,10 +245,16 @@ __device__ __forceinline__ float gemv_dot(int K, const float* wrow_f, const floa
     if (dbg && lane == 0) dbg[1] = (unsigned long long)clock64();
     return mine;
 }
+// weight row n of a [N, ldw] matrix of fp32 (WBF16 = false) or bf16 elements, as the pointer gemv_dot takes
+template <bool WBF16>
+__device__ __forceinline__ const float* gemv_wrow(const float* W, long long row_elems) {
+    if (WBF16) return reinterpret_cast<const float*>(reinterpret_cast<const unsigned short*>(W) + row_elems);
+    return W + row_elems;
+}
 
 // RAGGED (p.st heads a ragged state, `cur_pos` unused): a segment with pos_stride writes row b at the row's own cache position, and
 // leaves the cache of a finished row alone.
-template <int NB, bool W_GLOBAL, bool RAGGED = false>
+template <int NB, bool W_GLOBAL, bool RAGGED = false, bool WBF16 = false>
 __device__ __forceinline__ void gemv_row(const GemvParams& p, int n, const float* wrow_f, const float* xs, int b0, int lane, int cur_pos,
                                          bool have_operands = false, float bias_v = 0.f, float r_v = 0.f, unsigned long long* dbg = nullptr) {
     if (!have_operands) gemv_row_operands<NB>(p, n, b0, lane, bias_v, r_v);
@@ -249,7 +273,7 @@ __device__ __forceinline__ void gemv_row(const GemvParams& p, int n, const float
     const int act = sg.act;
     const float alpha = sg.alpha;
     const bool has_bias = p.bias != nullptr, has_res = p.R != nullptr;
-    const float mine = gemv_dot<NB, W_GLOBAL>(p.K, wrow_f, xs, lane, dbg);
+    const float mine = gemv_dot<NB, W_GLOBAL, WBF16>(p.K, wrow_f, xs, lane, dbg);
     if (lane < NB && b0 + lane < p.B) {
         float v = mine;
         if (has_bias) v += bias_v;

@@ -85,15 +85,20 @@ __device__ __forceinline__ float* wslice(float (&wbuf)[2][MEGA_WBUF_FLOATS], int
     return buf ? &wbuf[0][0] + 2 * MEGA_WBUF_FLOATS - floats : &wbuf[0][0];
 }
 
-// thread 0: start streaming this CTA's weight rows of GEMV phase `ph` into wbuf[buf]
+// floats of the arena a slice of `elems` weight elements takes (WBF16: two bf16 per float; K is a multiple of 8 there)
+template <bool WBF16>
+__device__ __forceinline__ int slice_floats(int elems) { return WBF16 ? elems >> 1 : elems; }
+
+// thread 0: start streaming this CTA's weight rows of GEMV phase `ph` into wbuf[buf] (WBF16: W holds bf16 bits, half the bytes)
+template <bool WBF16>
 __device__ __forceinline__ void prefetch_weights(const float* W, long long ldw, int N, int K, float* dst, unsigned long long* bar, int cta,
                                                  int rpc) {
     int r0, r1;
     cta_rows(N, cta, rpc, r0, r1);
-    const unsigned bytes = (unsigned)(r1 - r0) * (unsigned)K * 4u;
+    const unsigned bytes = (unsigned)(r1 - r0) * (unsigned)K * (WBF16 ? 2u : 4u);
     if (bytes == 0) { mbar_arrive(bar); return; }
     mbar_arrive_expect_tx(bar, bytes);
-    bulk_g2s(dst, W + (long long)r0 * ldw, bytes, bar);
+    bulk_g2s(dst, gemv_wrow<WBF16>(W, (long long)r0 * ldw), bytes, bar);
 }
 
 __device__ __forceinline__ bool wait_weights(unsigned long long* bar, unsigned parity, int* error_flag) {
@@ -136,8 +141,9 @@ __device__ __forceinline__ void grid_wait(unsigned int* counter, unsigned int ta
     __syncthreads();
 }
 
-// TRACE = true is a separate instantiation used only by the phase-timeline tool: the production kernel carries no stamp code
-template <int MEGA_NB, bool TRACE>
+// TRACE = true is a separate instantiation used only by the phase-timeline tool: the production kernel carries no stamp code.
+// WBF16: the phase table's weight matrices are the bf16 store (same rows per CTA, same prefetch schedule, half the bytes per slice).
+template <int MEGA_NB, bool TRACE, bool WBF16 = false>
 __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_megakernel(MegaParams mp) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     MegaSmem& sm = *reinterpret_cast<MegaSmem*>(smem_raw);
@@ -155,7 +161,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_megakernel(MegaParams 
     unsigned int sync_target = 0;
     if (tid == 0) {
         const MegaPhase* f = &mp.phases[mp.first_gemv];
-        prefetch_weights(f->g.W, f->g.ldw, f->g.N, f->g.K, wslice(sm.wbuf, 0, 0), &sm.mbar[0], cta, (f->g.N + G - 1) / G);
+        prefetch_weights<WBF16>(f->g.W, f->g.ldw, f->g.N, f->g.K, wslice(sm.wbuf, 0, 0), &sm.mbar[0], cta, (f->g.N + G - 1) / G);
     }
 
     // phase descriptors are double-buffered in shared memory: slot `cur` is the phase being executed, slot `cur ^ 1` is
@@ -251,7 +257,9 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_megakernel(MegaParams 
                 // queues this phase's few small latency-critical loads (activations, LN affine, bias) behind it.  It still has
                 // the rest of this phase plus the next prologue to land.
                 // issued by the LAST warp (it owns the fewest rows), from fields already in shared memory
-                if (tid == MEGA_THREADS - 32) prefetch_weights(ph.nx_W, ph.nx_ldw, ph.nx_N, ph.nx_K, wslice(sm.wbuf, buf ^ 1, ph.nx_rpc * ph.nx_K), &sm.mbar[buf ^ 1], cta, ph.nx_rpc);
+                if (tid == MEGA_THREADS - 32)
+                    prefetch_weights<WBF16>(ph.nx_W, ph.nx_ldw, ph.nx_N, ph.nx_K, wslice(sm.wbuf, buf ^ 1, slice_floats<WBF16>(ph.nx_rpc * ph.nx_K)), &sm.mbar[buf ^ 1],
+                                            cta, ph.nx_rpc);
                 wait_weights(&sm.mbar[buf], (g_idx >> 1) & 1, mp.error_flag);   // on a timeout the error flag ends the loop at the next token
                 MEGA_TRACE(3);
                 for (int rep = tracing ? 0 : 1; rep < 2; ++rep) {      // trace mode: a cold pass (stamp 12) and a warm one; idempotent, the
@@ -262,7 +270,8 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_megakernel(MegaParams 
                         const bool pre = j < OPS_ROWS;
                         const float bias_v = __shfl_sync(0xffffffffu, bias_pref, (j * MEGA_NB) & 31);
                         const float r_v = __shfl_sync(0xffffffffu, r_pref, (j * MEGA_NB + (lane < MEGA_NB ? lane : 0)) & 31);
-                        gemv_row<MEGA_NB, false>(ph.g, n, wslice(sm.wbuf, buf, ph.rpc * ph.g.K) + (long long)(n - r0) * ph.g.K, sm.u.xs, 0, lane, cur_pos, pre, bias_v, r_v,
+                        gemv_row<MEGA_NB, false, false, WBF16>(ph.g, n, gemv_wrow<WBF16>(wslice(sm.wbuf, buf, slice_floats<WBF16>(ph.rpc * ph.g.K)), (long long)(n - r0) * ph.g.K),
+                                                               sm.u.xs, 0, lane, cur_pos, pre, bias_v, r_v,
                                                  (tracing && warp == 0 && rep == 1 && j == 0) ? &mp.trace[(long long)pi * MEGA_TRACE_SLOTS + 13] : nullptr);
                     }
                 }
@@ -303,26 +312,32 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_megakernel(MegaParams 
 
 size_t mega_smem_bytes() { return sizeof(MegaSmem) + 128; }
 
-int launch_megakernel(const MegaParams& mp, int grid, cudaStream_t stream) {
+template <bool WBF16>
+static int launch_megakernel_impl(const MegaParams& mp, int grid, cudaStream_t stream) {
     static bool configured = false;
     if (!configured) {
-        MB_CUDA_CHECK(cudaFuncSetAttribute(decode_megakernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mega_smem_bytes()));
-        MB_CUDA_CHECK(cudaFuncSetAttribute(decode_megakernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mega_smem_bytes()));
-        MB_CUDA_CHECK(cudaFuncSetAttribute(decode_megakernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mega_smem_bytes()));
-        MB_CUDA_CHECK(cudaFuncSetAttribute(decode_megakernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mega_smem_bytes()));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(decode_megakernel<1, false, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mega_smem_bytes()));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(decode_megakernel<2, false, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mega_smem_bytes()));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(decode_megakernel<1, true, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mega_smem_bytes()));
+        MB_CUDA_CHECK(cudaFuncSetAttribute(decode_megakernel<2, true, WBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mega_smem_bytes()));
         int per_sm = 0;
-        MB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_megakernel<2, true>, MEGA_THREADS, mega_smem_bytes()));
+        MB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_megakernel<2, true, WBF16>, MEGA_THREADS, mega_smem_bytes()));
         MB_REQUIRE(per_sm >= 1, "megakernel does not fit on an SM");
         configured = true;
     }
     MB_REQUIRE(mp.sample.rows >= 1 && mp.sample.rows <= MEGA_NB_MAX, "megakernel handles 1 or 2 decoder rows");
     MegaParams p = mp;
     void* args[] = {&p};
-    const void* fn = mp.trace ? (mp.sample.rows == 1 ? (const void*)decode_megakernel<1, true> : (const void*)decode_megakernel<2, true>)
-                              : (mp.sample.rows == 1 ? (const void*)decode_megakernel<1, false> : (const void*)decode_megakernel<2, false>);
+    const void* fn = mp.trace ? (mp.sample.rows == 1 ? (const void*)decode_megakernel<1, true, WBF16> : (const void*)decode_megakernel<2, true, WBF16>)
+                              : (mp.sample.rows == 1 ? (const void*)decode_megakernel<1, false, WBF16> : (const void*)decode_megakernel<2, false, WBF16>);
     MB_CUDA_CHECK(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(MEGA_THREADS), args, mega_smem_bytes(), stream));
     ++g_launch_count;
+    if (WBF16) ++g_wbf16_launch_count;
     return 0;
+}
+
+int launch_megakernel(const MegaParams& mp, int grid, cudaStream_t stream, bool w_bf16) {
+    return w_bf16 ? launch_megakernel_impl<true>(mp, grid, stream) : launch_megakernel_impl<false>(mp, grid, stream);
 }
 
 }  // namespace mb200

@@ -99,13 +99,18 @@ __device__ __forceinline__ void cta_rows(int N, int cta, int rpc, int& r0, int& 
 __device__ __forceinline__ float* wslice(float (&wbuf)[2][MEGA_WBUF_FLOATS], int buf, int floats) {
     return buf ? &wbuf[0][0] + 2 * MEGA_WBUF_FLOATS - floats : &wbuf[0][0];
 }
+// floats of the arena a slice of `elems` weight elements takes (WBF16: two bf16 per float; K is a multiple of 8 there)
+template <bool WBF16>
+__device__ __forceinline__ int slice_floats(int elems) { return WBF16 ? elems >> 1 : elems; }
+// WBF16: W holds bf16 bits; the slice is the same rows at half the bytes
+template <bool WBF16>
 __device__ __forceinline__ void prefetch_weights(const float* W, long long ldw, int N, int K, float* dst, unsigned long long* bar, int cta, int rpc) {
     int r0, r1;
     cta_rows(N, cta, rpc, r0, r1);
-    const unsigned bytes = (unsigned)(r1 - r0) * (unsigned)K * 4u;
+    const unsigned bytes = (unsigned)(r1 - r0) * (unsigned)K * (WBF16 ? 2u : 4u);
     if (bytes == 0 || (c_ll_debug & 1)) { mbar_arrive(bar); return; }
     mbar_arrive_expect_tx(bar, bytes);
-    bulk_g2s(dst, W + (long long)r0 * ldw, bytes, bar);
+    bulk_g2s(dst, gemv_wrow<WBF16>(W, (long long)r0 * ldw), bytes, bar);
 }
 __device__ __forceinline__ bool wait_weights(unsigned long long* bar, unsigned parity, int* error_flag) {
     for (long long spin = 0; spin < (1ll << 24); ++spin)
@@ -421,19 +426,22 @@ __device__ __forceinline__ M3Map m3_make_map(int K, int tid) {
 // All row slots of the phase in one go (P = 8, 16 or 32 slots): weights are loaded in chunks of 8 rows (8 x LDS.128 in flight, branch-free:
 // out-of-range rows re-read row 0 and are discarded by a select), every row slot keeps its own accumulator, and ONE butterfly reduces
 // all of them at the end.  A phase is a chain of dependent latencies: one shuffle chain per phase instead of one per 8 rows.
-template <int NB, int P>
+// WBF16: the slice holds bf16 rows; column group kqc is read as 8 bytes and widened (the same products in the same order)
+template <int NB, int P, bool WBF16 = false>
 __device__ __forceinline__ void m3_rows(const float* wb, int K, int R, int G, int rg, int NS, const int (&kqc)[M3_NS], const float4 (&xv)[NB][M3_NS],
                                         float* red_b0, float* red_b1, int wi, int lane) {
     float acc[NB][P];
 #pragma unroll
     for (int c = 0; c < P / 8; ++c) {
         const float4* wrow[8];
+        const uint2* wrow16[8];
         bool valid[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
             const int lr = (c * 8 + i) * G + rg;
             valid[i] = lr < R;
-            wrow[i] = reinterpret_cast<const float4*>(wb + (valid[i] ? lr : 0) * K);
+            if constexpr (WBF16) wrow16[i] = reinterpret_cast<const uint2*>(reinterpret_cast<const unsigned short*>(wb) + (valid[i] ? lr : 0) * K);
+            else wrow[i] = reinterpret_cast<const float4*>(wb + (valid[i] ? lr : 0) * K);
 #pragma unroll
             for (int b = 0; b < NB; ++b) acc[b][c * 8 + i] = 0.f;
         }
@@ -443,7 +451,10 @@ __device__ __forceinline__ void m3_rows(const float* wb, int K, int R, int G, in
                 if (s < NS) {
                     float4 w[8];
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) w[i] = wrow[i][kqc[s]];
+                    for (int i = 0; i < 8; ++i) {
+                        if constexpr (WBF16) w[i] = bf16x4_to_float4(wrow16[i][kqc[s]]);
+                        else w[i] = wrow[i][kqc[s]];
+                    }
 #pragma unroll
                     for (int i = 0; i < 8; ++i)
 #pragma unroll
@@ -490,7 +501,7 @@ __device__ __forceinline__ M3Poll m3_make_poll(const MegaLL& ll, const M3Map& md
 // float4 product — gemv_dot's arithmetic and summation order, i.e. the same bits as the per-phase kernels and the barrier megakernel —
 // five shuffles per row, and the warp finishes its own rows (lane = row slot x replica: one store instruction writes every replica).
 // No cross-warp reduction, no epilogue hand-over: the phase's only CTA barrier is the one that publishes the activation.
-template <int NB, typename SM>
+template <int NB, bool WBF16, typename SM>
 __device__ __forceinline__ void m3_rw_tail(const Mega2Params& mp, const Mega2Phase& ph2, SM& sm, int cta, int tid, int buf, unsigned g_idx, int par,
                                            unsigned in_tag, unsigned out_tag, int cur_pos, int* err, unsigned long long* trace,
                                            ll_t (&w)[NB][M3_NS][4], const bool (&on)[NB][M3_NS], bool poller, const ll_t* in, int r0, int R) {
@@ -629,7 +640,9 @@ __device__ __forceinline__ void m3_rw_tail(const Mega2Params& mp, const Mega2Pha
 #pragma unroll
             for (int b = 0; b < NB; ++b) xr[b][j] = (j < nx && col < K4 && b < mp.rows) ? xs4[b * K4 + col] : make_float4(0, 0, 0, 0);
         }
-        const float4* wb4 = reinterpret_cast<const float4*>(wslice(sm.wbuf, buf, ph.rpc * K));
+        const float* wbs = wslice(sm.wbuf, buf, slice_floats<WBF16>(ph.rpc * K));
+        const float4* wb4 = reinterpret_cast<const float4*>(wbs);
+        const uint2* wb2 = reinterpret_cast<const uint2*>(wbs);
         float4 acc[NB][4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
@@ -638,11 +651,14 @@ __device__ __forceinline__ void m3_rw_tail(const Mega2Params& mp, const Mega2Pha
             const int row = warp + M2_WARPS * i;
             if (row < R) {                                 // warp-uniform
                 const float4* wrow = wb4 + row * K4;
+                const uint2* wrow2 = wb2 + row * K4;
 #pragma unroll
                 for (int j = 0; j < XS; ++j) {
                     if (j < nx) {
                         const int col = j * 32 + lane;
-                        const float4 wv = wrow[col < K4 ? col : 0];      // (x is zero beyond K4)
+                        float4 wv;                                       // (x is zero beyond K4)
+                        if constexpr (WBF16) wv = bf16x4_to_float4(wrow2[col < K4 ? col : 0]);
+                        else wv = wrow[col < K4 ? col : 0];
 #pragma unroll
                         for (int b = 0; b < NB; ++b) {
                             acc[b][i].x = fmaf(wv.x, xr[b][j].x, acc[b][i].x); acc[b][i].y = fmaf(wv.y, xr[b][j].y, acc[b][i].y);
@@ -679,7 +695,7 @@ __device__ __forceinline__ void m3_rw_tail(const Mega2Params& mp, const Mega2Pha
     if (trace && tid == 0) { trace[8] = (unsigned long long)clock64(); trace[9] = trace[8]; }
 }
 
-template <int NB, typename SM>
+template <int NB, bool WBF16, typename SM>
 __device__ __forceinline__ void m3_gemv_phase(const Mega2Params& mp, const Mega2Phase& ph2, SM& sm, const M3Map& mapd, const M3Map& mapf, const M3Poll& pl, int cta,
                                               int tid, unsigned g_idx, int par, unsigned in_tag, unsigned out_tag, int cur_pos, int* err,
                                               unsigned long long* trace /* null or [16] */) {
@@ -727,10 +743,11 @@ __device__ __forceinline__ void m3_gemv_phase(const Mega2Params& mp, const Mega2
     // it is done with it (a whole phase of lead for the copy).
     if (tid == M2_THREADS - 32) {
         if (g_idx > 0) wait_weights(&sm.wfree[buf ^ 1], ((g_idx - 1) >> 1) & 1, err);      // every warp has finished reading the slice of GEMV phase g_idx - 1
-        prefetch_weights(ph.nx_W, ph.nx_ldw, ph.nx_N, ph.nx_K, wslice(sm.wbuf, buf ^ 1, ph.nx_rpc * ph.nx_K), &sm.mbar[buf ^ 1], cta, ph.nx_rpc);
+        prefetch_weights<WBF16>(ph.nx_W, ph.nx_ldw, ph.nx_N, ph.nx_K, wslice(sm.wbuf, buf ^ 1, slice_floats<WBF16>(ph.nx_rpc * ph.nx_K)), &sm.mbar[buf ^ 1], cta,
+                                ph.nx_rpc);
     }
     if (isd) {
-        m3_rw_tail<NB>(mp, ph2, sm, cta, tid, buf, g_idx, par, in_tag, out_tag, cur_pos, err, trace, w, on, poller, in, r0, R);
+        m3_rw_tail<NB, WBF16>(mp, ph2, sm, cta, tid, buf, g_idx, par, in_tag, out_tag, cur_pos, err, trace, w, on, poller, in, r0, R);
         return;
     }
     const bool has_col = in_group && kq0 < K4;
@@ -878,15 +895,15 @@ __device__ __forceinline__ void m3_gemv_phase(const Mega2Params& mp, const Mega2
     // ---- multiply + reduce ----
     if (R > 0 && active_warp && !(c_ll_debug & 4)) {
         const int Pn = G == 1 ? R : (G == 2 ? (R + 1) >> 1 : (R + G - 1) / G);       // row slots per thread (host guarantees <= M3_SLOTS)
-        const float* wb = wslice(sm.wbuf, buf, ph.rpc * K);
+        const float* wb = wslice(sm.wbuf, buf, slice_floats<WBF16>(ph.rpc * K));
         int kqc[M3_NS];
 #pragma unroll
         for (int s = 0; s < M3_NS; ++s) kqc[s] = kq0 + s * M2_THREADS < K4 ? kq0 + s * M2_THREADS : 0;
         float* red0 = &sm.red[par][0][0][0];
         float* red1 = &sm.red[par][NB - 1][0][0];
-        if (Pn <= 8)       m3_rows<NB, 8>(wb, K, R, G, rg, NS, kqc, xv, red0, red1, wi, lane);
-        else if (Pn <= 16) m3_rows<NB, 16>(wb, K, R, G, rg, NS, kqc, xv, red0, red1, wi, lane);
-        else               m3_rows<NB, 32>(wb, K, R, G, rg, NS, kqc, xv, red0, red1, wi, lane);
+        if (Pn <= 8)       m3_rows<NB, 8, WBF16>(wb, K, R, G, rg, NS, kqc, xv, red0, red1, wi, lane);
+        else if (Pn <= 16) m3_rows<NB, 16, WBF16>(wb, K, R, G, rg, NS, kqc, xv, red0, red1, wi, lane);
+        else               m3_rows<NB, 32, WBF16>(wb, K, R, G, rg, NS, kqc, xv, red0, red1, wi, lane);
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(&sm.wfree[buf]);        // this warp no longer reads the weight slice
@@ -922,7 +939,8 @@ __device__ __forceinline__ void m3_gemv_phase(const Mega2Params& mp, const Mega2
 
 // TRACE = true is a separate instantiation for tools/mega2_trace.py: CTAs 0, 1, 100 and 140 stamp clock64 at four points of every phase
 // of token `trace_step` (phase start, input staged, weights landed, rows / units done); the production kernel carries no stamp code.
-template <int NB, bool TRACE>
+// WBF16: the phase table's weight matrices are the bf16 store (same rows per CTA, same schedule, half the bytes per slice)
+template <int NB, bool TRACE, bool WBF16 = false>
 __global__ void __launch_bounds__(M2_THREADS, 1) decode_megakernel_ll(Mega2Params mp) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     M2Smem& sm = *reinterpret_cast<M2Smem*>(smem_raw);
@@ -946,7 +964,7 @@ __global__ void __launch_bounds__(M2_THREADS, 1) decode_megakernel_ll(Mega2Param
     unsigned int g_idx = 0;          // running index of GEMV phases (selects weight buffer + mbarrier parity)
     if (tid == 0) {
         const MegaPhase* f = &mp.phases[0].base;
-        prefetch_weights(f->g.W, f->g.ldw, f->g.N, f->g.K, wslice(sm.wbuf, 0, 0), &sm.mbar[0], cta, (f->g.N + G - 1) / G);
+        prefetch_weights<WBF16>(f->g.W, f->g.ldw, f->g.N, f->g.K, wslice(sm.wbuf, 0, 0), &sm.mbar[0], cta, (f->g.N + G - 1) / G);
     }
     // CTA 0 publishes the residual stream left by the prefill (plain memory, written by an earlier kernel) and the first token header
     // under the tag the first phase of step 0 expects: "last phase of step -1"
@@ -1003,7 +1021,7 @@ __global__ void __launch_bounds__(M2_THREADS, 1) decode_megakernel_ll(Mega2Param
                 // timeline (TRACE instantiation, CTA mp.trace_cta): 16 stamps per phase, see tools/mega3_trace.py
                 unsigned long long* tr = nullptr;
                 if (TRACE && mp.trace != nullptr && step == mp.trace_step && cta == mp.trace_cta) tr = mp.trace + (long long)pi * 16;
-                m3_gemv_phase<NB>(mp, ph2, sm, mapd, mapf, pl, cta, tid, g_idx, pi & 1, in_tag, out_tag, cur_pos, err, tr);
+                m3_gemv_phase<NB, WBF16>(mp, ph2, sm, mapd, mapf, pl, cta, tid, g_idx, pi & 1, in_tag, out_tag, cur_pos, err, tr);
                 ++g_idx;
             } else if (ph.kind == 1) {
                 const DecAttnParams& a = ph.a;
@@ -1063,9 +1081,9 @@ int mega2_set_debug(int bits) {
     return 0;
 }
 
-template <int NB, bool TRACE>
+template <int NB, bool TRACE, bool WBF16>
 static const void* m2_configure() {
-    const void* fn = (const void*)decode_megakernel_ll<NB, TRACE>;
+    const void* fn = (const void*)decode_megakernel_ll<NB, TRACE, WBF16>;
     static bool done = false;
     if (!done) {
         if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mega2_smem_bytes()) != cudaSuccess) return nullptr;
@@ -1076,18 +1094,22 @@ static const void* m2_configure() {
     return fn;
 }
 
-int launch_megakernel2(const Mega2Params& mp, int grid, cudaStream_t stream) {
+int launch_megakernel2(const Mega2Params& mp, int grid, cudaStream_t stream, bool w_bf16) {
     MB_REQUIRE(mp.rows >= 1 && mp.rows <= M2_NB_MAX, "megakernel handles 1 or 2 decoder rows");
     MB_REQUIRE(mp.n_phases <= 126, "tag layout holds at most 126 phases per token");
     MB_REQUIRE(mp.d_model <= 1024, "residual scratch holds d_model <= 1024");
     const bool tr = mp.trace != nullptr, one = mp.rows == 1;
-    const void* fn = tr ? (one ? m2_configure<1, true>() : m2_configure<2, true>()) : (one ? m2_configure<1, false>() : m2_configure<2, false>());
+    const void* fn = w_bf16 ? (tr ? (one ? m2_configure<1, true, true>() : m2_configure<2, true, true>())
+                                  : (one ? m2_configure<1, false, true>() : m2_configure<2, false, true>()))
+                            : (tr ? (one ? m2_configure<1, true, false>() : m2_configure<2, true, false>())
+                                  : (one ? m2_configure<1, false, false>() : m2_configure<2, false, false>()));
     MB_REQUIRE(fn != nullptr, "dataflow megakernel does not fit on an SM");
     Mega2Params p = mp;
     void* args[] = {&p};
     // Cooperative launch for its co-residency guarantee: every CTA polls values that other CTAs produce, so all of them must be resident.
     MB_CUDA_CHECK(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(M2_THREADS), args, mega2_smem_bytes(), stream));
     ++g_launch_count;
+    if (w_bf16) ++g_wbf16_launch_count;
     return 0;
 }
 

@@ -9,6 +9,7 @@
 #include <memory>
 #include <tuple>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "../../include/mapperatorinator_b200.h"
@@ -39,6 +40,9 @@ struct LayerW {   // device pointers into the weight arena
     const float *ln1_w, *ln1_b, *wqkv, *bqkv, *wo, *bo;
     const float *ln2_w, *ln2_b, *wq_c, *bq_c, *wkv_c, *bkv_c, *wo_c, *bo_c;   // decoder cross attention only
     const float *ln3_w, *ln3_b, *fc1_w, *fc1_b, *fc2_w, *fc2_b;
+    // decoder only: the same packed matrices in the bf16 token-loop arena (bf16 bits behind a float pointer, as GemvParams::W carries
+    // them), null when the engine has no bf16 store
+    const float *wqkv16, *wo16, *wq_c16, *wo_c16, *fc1_w16, *fc2_w16;
 };
 
 }  // namespace
@@ -47,9 +51,12 @@ struct mb200_model {
     mb200_model_config cfg;
     MelPlan* mel = nullptr;
     std::unordered_map<std::string, std::vector<float>> host_w;   // until finalize()
+    std::unordered_set<std::string> bf16_names;                   // weights that arrived as bf16 (until finalize())
     bool finalized = false;
 
     DevBuf arena;                       // all packed weights
+    DevBuf arena16;                     // bf16 copies of the token loop's GEMV matrices (empty: the token loop reads the fp32 arena)
+    const float* proj_out16 = nullptr;  // bf16 bits of proj_out in arena16
     const float *emb_w = nullptr, *emb_b = nullptr, *conv1_w = nullptr, *conv1_b = nullptr, *conv2_w = nullptr, *conv2_b = nullptr,
                 *enc_pos = nullptr, *enc_ln_w = nullptr, *enc_ln_b = nullptr;
     const float *tok_emb = nullptr, *dec_pos = nullptr, *dec_ln_w = nullptr, *dec_ln_b = nullptr, *proj_out = nullptr;
@@ -280,6 +287,27 @@ extern "C" int mb200_model_set_weight(mb200_model* m, const char* name, const fl
     MB_REQUIRE(m && name && data, "null argument");
     MB_REQUIRE(!m->finalized, "model already finalized");
     m->host_w[name] = std::vector<float>(data, data + numel);
+    m->bf16_names.erase(name);
+    return 0;
+}
+
+extern "C" int mb200_model_set_weight_bf16(mb200_model* m, const char* name, const uint16_t* bits, int64_t numel) {
+    MB_REQUIRE(m && name && bits, "null argument");
+    MB_REQUIRE(!m->finalized, "model already finalized");
+    std::vector<float> w((size_t)numel);
+    for (int64_t i = 0; i < numel; ++i) {       // widening bf16 to fp32 is exact: the bits move to the top half
+        const uint32_t u = (uint32_t)bits[i] << 16;
+        std::memcpy(&w[(size_t)i], &u, 4);
+    }
+    m->host_w[name] = std::move(w);
+    m->bf16_names.insert(name);
+    return 0;
+}
+
+extern "C" int mb200_model_token_weight_bytes(const mb200_model* m, int32_t* bytes) {
+    MB_REQUIRE(m && bytes, "null argument");
+    MB_REQUIRE(m->finalized, "model not finalized");
+    *bytes = m->arena16.p ? 2 : 4;
     return 0;
 }
 
@@ -378,7 +406,54 @@ extern "C" int mb200_model_finalize(mb200_model* m) {
     };
     for (auto& o : eo) m->enc.push_back(fill(o, false));
     for (auto& o : dof) m->dec.push_back(fill(o, true));
+    // ---- bf16 store of the token loop's GEMV matrices ----
+    // Only when every matrix the token loop streams arrived as bf16 and every packed element (the q rows carry the folded 0.125) is
+    // still a bf16 value: the bf16 GEMV widens each element and sums in the fp32 kernel's order, so both stores give the same bits.
+    // The fp32 arena stays whole: the prefill GEMMs, the cross K/V projection and the teacher-forced passes read it.
+    {
+        std::vector<std::string> src = {"transformer.proj_out.weight"};
+        for (int i = 0; i < c.decoder_layers; ++i) {
+            const std::string p = "transformer.model.decoder.layers." + std::to_string(i) + ".";
+            for (const char* n : {"self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight", "self_attn.out_proj.weight",
+                                  "encoder_attn.q_proj.weight", "encoder_attn.out_proj.weight", "fc1.weight", "fc2.weight"})
+                src.push_back(p + n);
+        }
+        bool ok = d % 8 == 0 && f % 8 == 0;      // K of every matrix a multiple of 8: 16-byte rows for the 8-byte loads and bulk copies
+        for (const auto& n : src) ok = ok && m->bf16_names.count(n) == 1;
+        // (offset, element count) of every packed matrix in `pack`
+        std::vector<std::pair<size_t, size_t>> mats = {{o_proj, (size_t)c.vocab_size_out * d}};
+        for (const auto& o : dof) {
+            mats.push_back({o.v[2], (size_t)3 * d * d}); mats.push_back({o.v[4], (size_t)d * d}); mats.push_back({o.v[8], (size_t)d * d});
+            mats.push_back({o.v[12], (size_t)d * d}); mats.push_back({o.v[16], (size_t)f * d}); mats.push_back({o.v[18], (size_t)d * f});
+        }
+        std::vector<uint16_t> pack16;
+        std::vector<size_t> off16;
+        for (size_t k = 0; ok && k < mats.size(); ++k) {
+            const size_t o16 = (pack16.size() + 127) & ~size_t(127);      // 256-byte alignment
+            pack16.resize(o16 + mats[k].second);
+            for (size_t i = 0; i < mats[k].second; ++i) {
+                uint32_t u;
+                std::memcpy(&u, &pack[mats[k].first + i], 4);
+                if (u & 0xffffu) { ok = false; break; }
+                pack16[o16 + i] = (uint16_t)(u >> 16);
+            }
+            off16.push_back(o16);
+        }
+        if (ok) {
+            MB_TRY(m->arena16.ensure(pack16.size() * sizeof(uint16_t)));
+            MB_CUDA_CHECK(cudaMemcpy(m->arena16.p, pack16.data(), pack16.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
+            const uint16_t* b16 = m->arena16.as<uint16_t>();
+            auto at = [&](size_t k) { return reinterpret_cast<const float*>(b16 + off16[k]); };
+            m->proj_out16 = at(0);
+            for (size_t l = 0; l < m->dec.size(); ++l) {
+                LayerW& w = m->dec[l];
+                w.wqkv16 = at(1 + 6 * l); w.wo16 = at(2 + 6 * l); w.wq_c16 = at(3 + 6 * l);
+                w.wo_c16 = at(4 + 6 * l); w.fc1_w16 = at(5 + 6 * l); w.fc2_w16 = at(6 + 6 * l);
+            }
+        }
+    }
     m->host_w.clear();
+    m->bf16_names.clear();
     // tf32 "lo" mirrors of the weights that feed large (tensor-core) GEMMs: encoder stem + layers, cross K|V projections
     {
         const long long dd = (long long)d * d;
@@ -666,16 +741,23 @@ static GemvParams gemv_base(int xmode, const float* W, long long ldw, const floa
     return g;
 }
 
-static GemvParams final_logits_params(mb200_model* m, int rows, const float* x, long long x_ld) {
+// Does the token loop stream the bf16 store?  Whenever the engine holds one: measured (tools/bf16_bench.py, README) faster than the
+// fp32 copy on every driver and row count, megakernels and per-kernel GEMVs alike.
+static bool token_bf16(const mb200_model* m) { return m->arena16.p != nullptr; }
+
+// wbf: W is proj_out's bf16 copy (launch with w_bf16 = true)
+static GemvParams final_logits_params(mb200_model* m, int rows, const float* x, long long x_ld, bool wbf) {
     const auto& c = m->cfg;
-    GemvParams g = gemv_base(X_LAYERNORM, m->proj_out, c.d_model, nullptr, c.d_model, c.vocab_size_out, rows, m->g_state.as<GenState>());
+    GemvParams g = gemv_base(X_LAYERNORM, wbf ? m->proj_out16 : m->proj_out, c.d_model, nullptr, c.d_model, c.vocab_size_out, rows,
+                             m->g_state.as<GenState>());
     g.x = x; g.x_ld = x_ld; g.ln_w = m->dec_ln_w; g.ln_b = m->dec_ln_b;
     g.seg[0].out = m->d_logits.as<float>(); g.seg[0].out_bs = c.vocab_size_out;
     return g;
 }
 
 static int final_logits(mb200_model* m, int rows, const float* x, long long x_ld, cudaStream_t st, bool pdl) {
-    return launch_gemv(final_logits_params(m, rows, x, x_ld), st, pdl);
+    const bool wbf = token_bf16(m);
+    return launch_gemv(final_logits_params(m, rows, x, x_ld, wbf), st, pdl, false, GEMV_FORM_KERNEL, wbf);
 }
 
 static SampleParams sample_params(mb200_model* m, int rows) {
@@ -695,8 +777,12 @@ static SampleParams sample_params(mb200_model* m, int rows) {
 // ragged: the step of a ragged call (per-phase kernels only) — n_splits_self is then the largest self-attention plan of the call.
 static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaStream_t st, bool pdl,
                       std::vector<MegaPhase>* collect = nullptr, const BeamParams* beam = nullptr, bool ragged = false) {
+    // the weight store of this step's GEMVs (a megakernel's phase table carries it too)
+    const bool wbf = token_bf16(m);
+    auto TW = [&](const float* w32, const float* w16) { return wbf ? w16 : w32; };
     auto emit_gemv = [&](const GemvParams& g) -> int {
-        if (!collect) return launch_gemv(g, st, pdl, ragged && g.nseg > 1);      // only the cache-writing GEMV reads the row's position
+        // only the cache-writing GEMV reads the row's position
+        if (!collect) return launch_gemv(g, st, pdl, ragged && g.nseg > 1, GEMV_FORM_KERNEL, wbf);
         MegaPhase ph{}; ph.kind = 0; ph.g = g; collect->push_back(ph);
         return 0;
     };
@@ -721,7 +807,7 @@ static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaSt
         float* skv = m->self_kv.as<float>() + (size_t)l * m->self_layer_stride();
         const float* ckv = m->cross_kv.as<float>() + (size_t)l * m->cross_layer_stride();
         {   // LN1 -> q | k | v  (k, v land in the self cache at position cur_len - 1)
-            GemvParams g = gemv_base(X_LAYERNORM, w.wqkv, d, w.bqkv, d, 3 * d, rows, gs);
+            GemvParams g = gemv_base(X_LAYERNORM, TW(w.wqkv, w.wqkv16), d, w.bqkv, d, 3 * d, rows, gs);
             g.x = x; g.x_ld = d; g.ln_w = w.ln1_w; g.ln_b = w.ln1_b;
             g.nseg = 3;
             g.seg[0] = GemvSeg{q, d, 0, 0, d, 1.f, ACT_NONE};
@@ -744,13 +830,13 @@ static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaSt
             MB_TRY(emit_attn(a));
         }
         {   // out_proj + residual (the heads were merged by the attention phase)
-            GemvParams g = gemv_base(X_PLAIN, w.wo, d, w.bo, d, d, rows, gs);
+            GemvParams g = gemv_base(X_PLAIN, TW(w.wo, w.wo16), d, w.bo, d, d, rows, gs);
             g.x = attn; g.x_ld = d;
             g.seg[0].out = x; g.seg[0].out_bs = d; g.R = x; g.r_ld = d;
             MB_TRY(emit_gemv(g));
         }
         {   // LN2 -> cross q
-            GemvParams g = gemv_base(X_LAYERNORM, w.wq_c, d, w.bq_c, d, d, rows, gs);
+            GemvParams g = gemv_base(X_LAYERNORM, TW(w.wq_c, w.wq_c16), d, w.bq_c, d, d, rows, gs);
             g.x = x; g.x_ld = d; g.ln_w = w.ln2_w; g.ln_b = w.ln2_b;
             g.seg[0].out = q; g.seg[0].out_bs = d;
             MB_TRY(emit_gemv(g));
@@ -764,25 +850,25 @@ static int token_step(mb200_model* m, int rows, int B, int n_splits_self, cudaSt
             MB_TRY(emit_attn(a));
         }
         {
-            GemvParams g = gemv_base(X_PLAIN, w.wo_c, d, w.bo_c, d, d, rows, gs);
+            GemvParams g = gemv_base(X_PLAIN, TW(w.wo_c, w.wo_c16), d, w.bo_c, d, d, rows, gs);
             g.x = attn; g.x_ld = d;
             g.seg[0].out = x; g.seg[0].out_bs = d; g.R = x; g.r_ld = d;
             MB_TRY(emit_gemv(g));
         }
         {   // LN3 -> fc1 + GELU
-            GemvParams g = gemv_base(X_LAYERNORM, w.fc1_w, d, w.fc1_b, d, f, rows, gs);
+            GemvParams g = gemv_base(X_LAYERNORM, TW(w.fc1_w, w.fc1_w16), d, w.fc1_b, d, f, rows, gs);
             g.x = x; g.x_ld = d; g.ln_w = w.ln3_w; g.ln_b = w.ln3_b;
             g.seg[0] = GemvSeg{hh, f, 0, 0, f, 1.f, ACT_GELU_ERF};
             MB_TRY(emit_gemv(g));
         }
         {   // fc2 + residual
-            GemvParams g = gemv_base(X_PLAIN, w.fc2_w, f, w.fc2_b, f, d, rows, gs);
+            GemvParams g = gemv_base(X_PLAIN, TW(w.fc2_w, w.fc2_w16), f, w.fc2_b, f, d, rows, gs);
             g.x = hh; g.x_ld = f;
             g.seg[0].out = x; g.seg[0].out_bs = d; g.R = x; g.r_ld = d;
             MB_TRY(emit_gemv(g));
         }
     }
-    MB_TRY(emit_gemv(final_logits_params(m, rows, x, d)));
+    MB_TRY(emit_gemv(final_logits_params(m, rows, x, d, wbf)));
     if (collect) {
         MegaPhase ph{}; ph.kind = 2; collect->push_back(ph);
         const int n = (int)collect->size();
@@ -861,7 +947,7 @@ static int run_megakernel(mb200_model* m, int rows, int B, int n_splits_self, in
         mp.sync_counter = m->g_megasync.as<unsigned int>(); mp.error_flag = m->g_megasync.as<int>() + 8;
         mp.max_steps = max_steps; mp.row_slot = m->g_rowslot.as<int>();
         mp.trace = m->mega_trace.p ? m->mega_trace.as<unsigned long long>() : nullptr; mp.trace_step = 8;
-        return launch_megakernel(mp, m->num_sms, st);
+        return launch_megakernel(mp, m->num_sms, st, token_bf16(m));
     };
     MB_TRY(mega_launch(m, st, launch, before_sync));
     MB_REQUIRE(m->h_flag[1] == 0, m->h_flag[1] == 1 ? "megakernel grid barrier timed out" : "megakernel weight copy timed out");
@@ -922,7 +1008,7 @@ static int run_megakernel2(mb200_model* m, int rows, int B, int n_splits_self, i
         mp.max_steps = max_steps; mp.row_slot = m->g_rowslot.as<int>(); mp.x_in = m->d_x.as<float>();
         mp.rows = rows; mp.d_model = m->cfg.d_model; mp.V = m->cfg.vocab_size_out; mp.ffn_dim = m->cfg.ffn_dim; mp.trace_cta = m->trace_cta;
         mp.trace = m->mega_trace.p ? m->mega_trace.as<unsigned long long>() : nullptr; mp.trace_step = 8;
-        return launch_megakernel2(mp, m->num_sms, st);
+        return launch_megakernel2(mp, m->num_sms, st, token_bf16(m));
     };
     MB_TRY(mega_launch(m, st, launch, before_sync));
     if (m->h_flag[1] == 4) {
@@ -1276,9 +1362,10 @@ int stream_admit(mb200_stream* s, int n, const int32_t* slots, const int64_t* pr
     for (int j = 0; j < n; ++j) {
         const int P = prompt_off[j + 1] - prompt_off[j], r = list[j];
         MB_TRY(decoder_prefill(m, nr, P, m->g_prefill_ids.as<long long>() + pre_off[j], 0, st, r, N, rowslot + m->max_rows + 2 * r));
-        GemvParams g = final_logits_params(m, nr, m->p_x.as<float>() + (size_t)(P - 1) * d, (long long)P * d);
+        const bool wbf = token_bf16(m);
+        GemvParams g = final_logits_params(m, nr, m->p_x.as<float>() + (size_t)(P - 1) * d, (long long)P * d, wbf);
         g.seg[0].out += (size_t)r * V; g.seg[0].out_bs = (long long)N * V;
-        MB_TRY(launch_gemv(g, st, false));
+        MB_TRY(launch_gemv(g, st, false, false, GEMV_FORM_KERNEL, wbf));
     }
     // the list selection sets all_finished again if every row of the stream is finished after it
     MB_CUDA_CHECK(cudaMemsetAsync(&gs->all_finished, 0, sizeof(int), st));

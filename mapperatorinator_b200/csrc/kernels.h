@@ -238,7 +238,9 @@ struct GemvParams {
 // tests compare with KERNEL bit for bit.
 enum GemvForm : int { GEMV_FORM_KERNEL = 0, GEMV_FORM_MEGA = 1 };
 // ragged: p.st heads a ragged state; segments with pos_stride write row b at ITS cache position, and not at all once it has finished
-int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged = false, int form = GEMV_FORM_KERNEL);
+// w_bf16: p.W holds bf16 bits ([N, ldw] elements, K and ldw multiples of 8, 16-byte aligned); the sums are the bits of the fp32 kernel
+// on the widened weights
+int launch_gemv(const GemvParams& p, cudaStream_t stream, bool pdl, bool ragged = false, int form = GEMV_FORM_KERNEL, bool w_bf16 = false);
 
 struct DecAttnParams {
     const float* q; long long q_ld;                 // [rows, d_model], already scaled
@@ -333,7 +335,8 @@ struct MegaParams {
     int trace_step;
 };
 size_t mega_smem_bytes();
-int launch_megakernel(const MegaParams& mp, int grid, cudaStream_t stream);
+// w_bf16: the phase table carries the bf16 store
+int launch_megakernel(const MegaParams& mp, int grid, cudaStream_t stream, bool w_bf16 = false);
 
 // ---- decode_mega2.cu: the DATAFLOW token-loop megakernel ----------------------------------------------------------------
 // Same phases, same arithmetic, no grid barrier: every value that crosses CTAs travels as an 8-byte {fp32 bits | tag << 32} pair
@@ -382,7 +385,8 @@ struct Mega2Params {
     unsigned long long* trace; int trace_step, trace_cta;    // optional [n_phases][16] clock64 stamps of one CTA (tools/mega3_trace.py)
 };
 size_t mega2_smem_bytes();
-int launch_megakernel2(const Mega2Params& mp, int grid, cudaStream_t stream);
+// w_bf16: the phase table carries the bf16 store
+int launch_megakernel2(const Mega2Params& mp, int grid, cudaStream_t stream, bool w_bf16 = false);
 bool mega2_ksplit_ok(int N, int K, int rows, int grid);   // does one GEMV phase fit the K-split thread mapping?
 int mega2_set_debug(int bits);                    // diagnostics (decode_device.cuh, c_ll_debug)
 int mega2_set_poll_sleep(int ns);                 // tuning: nanoseconds to back off after a failed poll (0 = spin)

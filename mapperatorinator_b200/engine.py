@@ -102,9 +102,24 @@ class ModelEngine:
             for name, t in state_dict.items():
                 if not isinstance(t, torch.Tensor) or not t.is_floating_point():
                     continue
+                if t.dtype == torch.bfloat16:      # raw bits: the engine widens them and may serve the token loop from a bf16 store
+                    a = t.detach().to("cpu").contiguous().view(torch.int16).numpy()
+                    _lib.check(self.lib.mb200_model_set_weight_bf16(self.handle, name.encode(), a.ctypes.data, a.size))
+                    continue
                 a = t.detach().to("cpu", torch.float32).contiguous().numpy()
                 _lib.check(self.lib.mb200_model_set_weight(self.handle, name.encode(), a.ctypes.data, a.size))
             _lib.check(self.lib.mb200_model_finalize(self.handle))
+        nbytes = C.c_int32()
+        _lib.check(self.lib.mb200_model_token_weight_bytes(self.handle, C.byref(nbytes)))
+        self._token_weight_dtype = torch.bfloat16 if nbytes.value == 2 else torch.float32
+
+    @property
+    def token_weight_dtype(self) -> torch.dtype:
+        """torch.bfloat16 when the engine holds a bf16 token-loop store (every decoder GEMV matrix and proj_out arrived as bf16: a model
+        loaded at bf16 precision), else torch.float32.  Every token-loop driver then streams the bf16 store (megakernels, CUDA
+        graph, ragged, stream, beam).  The results are the same bits either way: bf16 weights are widened exactly and summed in the
+        fp32 order."""
+        return self._token_weight_dtype
 
     # ---- encoder ---------------------------------------------------------------------------------------------------
     def encode(self, pcm: torch.Tensor, slot_begin: int = 0, return_states: bool = False) -> Optional[torch.Tensor]:

@@ -125,10 +125,13 @@ def gemv(x, w, bias=None, *, ln_weight=None, ln_bias=None, eps=1e-5, xmode=None,
     (xmode "layernorm", or force either mode by name).  Without `segments` the output is one segment over [0, N) into `out` (allocated
     (B, N) when not given; it may be `residual` itself) and is returned.  `segments` (GemvSegment, 1 to 3) route the columns instead,
     positional ones at `cur_len` (or per request: ragged_cur_len / ragged_finished with rows r and r + n_req sharing request r).
-    form "kernel" is the per-phase kernel, "mega" the barrier megakernel's phase body."""
+    form "kernel" is the per-phase kernel, "mega" the barrier megakernel's phase body.  A bfloat16 `w` runs the bf16-weight GEMV of
+    the token loop's bf16 store (`mb200_op_gemv_bf16`: K and w's row stride multiples of 8, rows 16-byte aligned)."""
     import ctypes as C
     lib = _lib.load()
-    for t in (x, w, bias, ln_weight, ln_bias, residual, out):
+    w_bf16 = w.dtype == torch.bfloat16
+    assert w.is_cuda and w.stride(-1) == 1 and w.dtype in (torch.float32, torch.bfloat16)
+    for t in (x, bias, ln_weight, ln_bias, residual, out):
         assert t is None or (t.is_cuda and t.dtype == torch.float32 and t.stride(-1) == 1)
     B, K = x.shape
     N = w.shape[0]
@@ -145,7 +148,7 @@ def gemv(x, w, bias=None, *, ln_weight=None, ln_bias=None, eps=1e-5, xmode=None,
         n_req = len(ragged_cur_len) if n_req is None else n_req
         rc = (C.c_int32 * n_req)(*[int(v) for v in ragged_cur_len])
         rf = (C.c_int32 * n_req)(*[int(v) for v in ragged_finished])
-    _lib.check(lib.mb200_op_gemv(_ptr(x), x.stride(0), B, K, {"plain": 0, "layernorm": 1}[xmode], _ptr(ln_weight), _ptr(ln_bias), float(eps),
+    _lib.check((lib.mb200_op_gemv_bf16 if w_bf16 else lib.mb200_op_gemv)(_ptr(x), x.stride(0), B, K, {"plain": 0, "layernorm": 1}[xmode], _ptr(ln_weight), _ptr(ln_bias), float(eps),
                                  _ptr(w), w.stride(0), N, _ptr(bias), _ptr(residual), residual.stride(0) if residual is not None else 0,
                                  segs, len(segments), int(cur_len), None if rc is None else C.cast(rc, C.c_void_p),
                                  None if rf is None else C.cast(rf, C.c_void_p), int(n_req or 0), GEMV_FORMS[form], _stream()))

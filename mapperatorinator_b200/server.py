@@ -40,7 +40,10 @@ def _build_generation_stats(result: torch.Tensor, model_kwargs: dict, pad_token_
 @torch.no_grad()
 def model_generate(model, tokenizer, model_kwargs, generate_kwargs):
     """`model_generate(model, tokenizer, model_kwargs, generate_kwargs) -> (LongTensor[B, P+N] on CPU, stats)`.
-    `precision` is accepted for signature parity; the engine computes in fp32 (the parity contract of the hot path)."""
+    `precision` is accepted for signature parity and ignored: the engine computes in fp32 (the parity contract of the hot path), and
+    `precision='amp'` stays fp32.  The model's LOAD precision decides the weight store: a model loaded in bf16 (every decoder GEMV
+    matrix and proj_out bf16) has its token loop's per-kernel GEMVs read a bf16 copy of those weights, with the same ids as the same
+    values served from fp32 (`ModelEngine.token_weight_dtype`)."""
     generate_kwargs = dict(generate_kwargs)
     generate_kwargs.pop("precision", None)
     layout = TokenLayout.from_tokenizer(tokenizer)
@@ -181,7 +184,8 @@ def model_score(model, model_kwargs, generate_kwargs):
     """MaiMod's scoring of given tokens (processor.py:511-525) on the teacher-forced pass `model_forward` runs, reduced on the
     device: takes `model_forward`'s arguments and returns a dict of CPU tensors [B, L] indexed by the scored token (`entropy`,
     `surprisal`, `relative`, `suggested`; see `ModelEngine.score_tokens`), so the caller slices `[start + padding, end + padding)`
-    where it sliced the logits at `[start + padding - 1, end + padding - 1)`.  `precision` is accepted and ignored (fp32).
+    where it sliced the logits at `[start + padding - 1, end + padding - 1)`.  `precision` is accepted and ignored (fp32); the
+    teacher-forced pass reads the fp32 weights whatever precision the model was loaded in.
     A guided call (`cfg_scale > 1` with a negative prompt) is refused: the reference repeats the decoder rows but not the frames
     there, which is not a pass worth mirroring."""
     generate_kwargs = dict(generate_kwargs)
