@@ -288,19 +288,38 @@ int mb200_model_mega_stats(mb200_model* m, double* out, int32_t reset);
 /* ------------------------------------------------------------------------------------------------------------------
  * Kernel-level entry points (parity tests of the individual kernels; not needed by an integrator).
  * ------------------------------------------------------------------------------------------------------------------ */
-int mb200_op_gemm(const float* A, int64_t lda, const float* W, int64_t ldw, float* C, int64_t ldc, const float* bias, int32_t act,
-                  float alpha, const float* residual, int64_t ldr, const float* gate, int64_t gate_ld, int32_t gate_rpb, int32_t M,
-                  int32_t N, int32_t K, void* cuda_stream);
-/* the wgmma 3xTF32 GEMM on its own (registers W's lo mirror, runs, synchronises, checks the pipeline error flag) */
-int mb200_op_gemm_tc(const float* A, int64_t lda, const float* W, int64_t ldw, float* C, int64_t ldc, const float* bias, int32_t act,
-                     float alpha, const float* residual, int64_t ldr, int32_t M, int32_t N, int32_t K, void* cuda_stream);
+/* Rows of a matrix operand as the engine addresses them: logical row m at ptr + (m / rpb) * bstride + (m % rpb) * ld (rpb 0: ptr + m * ld).
+ * Rows may overlap (the conv stem reads a 3-tap window of a padded buffer as one row of 3 * ld floats) and bstride may be 0 (one table
+ * added to every batch item). */
+typedef struct mb200_rowmap {
+    float* ptr;
+    int64_t ld;
+    int32_t rpb;
+    int64_t bstride;
+} mb200_rowmap;
+/* One dense GEMM through the engine's own launch functions (gemm.cu / gemm_tc.cu):
+ *   C[m, n] = act(A[m, :] . W[n, :] + bias[n]) * alpha [* gate[(m / gate_rpb) * gate_ld + n]] [+ R[m, n]],  m < M, n < N
+ * A, C and R (null = none; it may be C itself) are row maps; W [N rows of K at stride ldw]; bias [N] or null.
+ * path 0: W gets a tf32 mirror as the engine's registered weights have, and the engine's dispatch picks the kernel; 1: no mirror, the
+ * fp32 SIMT kernel; 2: the wgmma 3xTF32 kernel, or an error if the problem is not eligible for it.  Every argument is checked before
+ * anything is launched.  All pointers are DEVICE.  Synchronises the stream and reports a pipeline time-out of the tensor-core path. */
+int mb200_op_gemm_mapped(const mb200_rowmap* A, const float* W, int64_t ldw, const mb200_rowmap* C, const float* bias, int32_t act,
+                         float alpha, const mb200_rowmap* R, const float* gate, int64_t gate_ld, int32_t gate_rpb, int32_t M, int32_t N,
+                         int32_t K, int32_t path, void* cuda_stream);
 /* 0 = route every GEMM through the fp32 SIMT kernel (A/B comparisons), 1 = tensor cores where eligible (default) */
 int mb200_set_tensor_cores(int32_t enabled);
-int mb200_op_layernorm(const float* x, float* y, const float* w, const float* b, const float* shift, const float* scale,
+/* LayerNorm of rows x [rows, dim] (contiguous) into y: affine with w / b, or the adaLN modulate y = LN(x) * (1 + scale) + shift with
+ * shift / scale rows of batch item m / rows_per_batch at stride mod_ld (0 = dim). */
+int mb200_op_layernorm(const float* x, float* y, const float* w, const float* b, const float* shift, const float* scale, int64_t mod_ld,
                        int32_t rows_per_batch, int32_t rows, int32_t dim, float eps, void* cuda_stream);
-int mb200_op_attention(const float* q, const float* k, const float* v, float* o, int32_t B, int32_t H, int32_t Tq, int32_t Tk,
-                       float scale, int32_t mask_mode, int32_t q_pos0, const uint8_t* key_valid, int32_t band,
-                       const uint8_t* dense_mask, void* cuda_stream);
+/* Dense attention (attention.cu / attention_tc.cu), head_dim 64: element (b, t, h, d) of q / k / v / o at ptr + b * bs + t * ld + h * 64 + d.
+ * key_valid [B rows of key_valid_ld] (1 = real key) or null; kv_slot (DEVICE int32 [B], or null): batch row b reads K / V of batch index
+ * kv_slot[b].  mask_mode 0 none, 1 causal (query t sees keys <= q_pos0 + t), 2 band, 3 dense [Tq, Tk] (1 = blocked).
+ * The tensor-core path runs where it is eligible (see mb200_set_attention_tc). */
+int mb200_op_attention(const float* q, int64_t q_ld, int64_t q_bs, const float* k, int64_t k_ld, int64_t k_bs, const float* v, int64_t v_ld,
+                       int64_t v_bs, float* o, int64_t o_ld, int64_t o_bs, int32_t B, int32_t H, int32_t Tq, int32_t Tk, float scale,
+                       int32_t mask_mode, int32_t q_pos0, const uint8_t* key_valid, int64_t key_valid_ld, int32_t band,
+                       const uint8_t* dense_mask, const int32_t* kv_slot, void* cuda_stream);
 /* One split-KV decode-attention phase of the token loop (decode.cu), through the engine's own launch functions and split plan.
  * q [rows, H*64] already scaled; kv: K|V cache [slots, t_max, 2*H*64] (token stride 2*H*64, V at offset H*64); row_slot [rows] cache
  * row of each decoder row (null = row r); out [rows, H*64] merged heads.  All pointers are DEVICE except ragged_cur_len /

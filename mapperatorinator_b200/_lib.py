@@ -46,6 +46,10 @@ class GemvSegC(C.Structure):
                 ("alpha", C.c_float), ("act", C.c_int32)]
 
 
+class RowMapC(C.Structure):
+    _fields_ = [("ptr", C.c_void_p), ("ld", C.c_int64), ("rpb", C.c_int32), ("bstride", C.c_int64)]
+
+
 class DitMaskC(C.Structure):
     _fields_ = [("mask_mode", C.c_int32), ("band", C.c_int32), ("dense_mask", C.c_void_p)]
 
@@ -63,7 +67,7 @@ ABI_SYMBOLS = [
     "mb200_dit_sample_loop", "mb200_dit_set_option", "mb200_dit_set_sliders", "mb200_dit_apply_sliders",
     "mb200_launch_count", "mb200_wbf16_launch_count", "mb200_model_set_option", "mb200_model_profile_step", "mb200_model_read_trace", "mb200_model_mega_stats", "mb200_model_logits_chain",
     "mb200_model_beam_step",
-    "mb200_op_gemm", "mb200_op_gemm_tc", "mb200_set_tensor_cores", "mb200_op_layernorm", "mb200_op_attention", "mb200_op_decode_attention", "mb200_op_gemv", "mb200_op_gemv_bf16", "mb200_set_attention_tc", "mb200_audio_out_frames", "mb200_audio_ingest",
+    "mb200_op_gemm_mapped", "mb200_set_tensor_cores", "mb200_op_layernorm", "mb200_op_attention", "mb200_op_decode_attention", "mb200_op_gemv", "mb200_op_gemv_bf16", "mb200_set_attention_tc", "mb200_audio_out_frames", "mb200_audio_ingest",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -120,11 +124,12 @@ def load() -> C.CDLL:
     lib.mb200_dit_set_option.argtypes = [vp, C.c_char_p, i32]
     lib.mb200_dit_set_sliders.argtypes = [vp, i32, vp, vp, vp, vp, vp]
     lib.mb200_dit_apply_sliders.argtypes = [vp, vp, i32, i32, vp]
-    lib.mb200_op_gemm.argtypes = [vp, i64, vp, i64, vp, i64, vp, i32, f32, vp, i64, vp, i64, i32, i32, i32, i32, vp]
-    lib.mb200_op_gemm_tc.argtypes = [vp, i64, vp, i64, vp, i64, vp, i32, f32, vp, i64, i32, i32, i32, vp]
+    rm = C.POINTER(RowMapC)
+    lib.mb200_op_gemm_mapped.argtypes = [rm, vp, i64, rm, vp, i32, f32, rm, vp, i64, i32, i32, i32, i32, i32, vp]
     lib.mb200_set_tensor_cores.argtypes = [i32]
-    lib.mb200_op_layernorm.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, vp]
-    lib.mb200_op_attention.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, f32, i32, i32, vp, i32, vp, vp]
+    lib.mb200_op_layernorm.argtypes = [vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, f32, vp]
+    lib.mb200_op_attention.argtypes = [vp, i64, i64, vp, i64, i64, vp, i64, i64, vp, i64, i64, i32, i32, i32, i32, f32, i32, i32, vp, i64,
+                                       i32, vp, vp, vp]
     lib.mb200_set_attention_tc.argtypes = [i32, i32]
     lib.mb200_op_decode_attention.argtypes = [vp, vp, i32, i32, i32, i32, vp, i32, i32, vp, i64, i32, i32, vp, i64, vp, vp, i32, vp, vp]
     lib.mb200_op_gemv.argtypes = [vp, i64, i32, i32, i32, vp, vp, f32, vp, i64, i32, vp, vp, i64, C.POINTER(GemvSegC), i32, i32, vp, vp,

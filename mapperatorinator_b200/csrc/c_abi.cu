@@ -16,6 +16,7 @@ StepProfiler g_prof;
 }  // namespace mb200
 
 using namespace mb200;
+#define OP_TRY(expr) do { int _s = (expr); if (_s) return _s; } while (0)
 
 struct mb200_mel {
     MelPlan* plan;
@@ -49,33 +50,46 @@ extern "C" int mb200_mel_forward(mb200_mel* mel, const float* pcm, int32_t batch
                       (cudaStream_t)stream);
 }
 
-extern "C" int mb200_op_gemm(const float* A, int64_t lda, const float* W, int64_t ldw, float* C, int64_t ldc, const float* bias, int32_t act,
-                             float alpha, const float* residual, int64_t ldr, const float* gate, int64_t gate_ld, int32_t gate_rpb, int32_t M,
-                             int32_t N, int32_t K, void* stream) {
+// One dense GEMM through the engine's own launch functions, with GemmParams filled from row maps as the encoder, the decoder prefill and
+// the DiT fill them.  path 0: W gets a tf32 mirror as finalize gives the weights it registers, and launch_gemm picks what the engine would
+// pick; 1: no mirror, so launch_gemm runs the fp32 SIMT kernel; 2: launch_gemm_tc, or an error naming why the problem is not eligible.
+extern "C" int mb200_op_gemm_mapped(const mb200_rowmap* A, const float* W, int64_t ldw, const mb200_rowmap* C, const float* bias, int32_t act,
+                                    float alpha, const mb200_rowmap* R, const float* gate, int64_t gate_ld, int32_t gate_rpb, int32_t M,
+                                    int32_t N, int32_t K, int32_t path, void* stream) {
+    MB_REQUIRE(A && A->ptr && W && C && C->ptr && (!R || R->ptr), "null argument");
+    MB_REQUIRE(path >= 0 && path <= 2, "path is 0 (engine dispatch), 1 (SIMT) or 2 (tensor cores)");
+    MB_REQUIRE(M >= 1 && N >= 1 && K >= 4 && K % 4 == 0, "need M >= 1, N >= 1 and K a positive multiple of 4");
+    MB_REQUIRE(act >= ACT_NONE && act <= ACT_SILU, "unknown activation");
+    for (const mb200_rowmap* m : {A, C, R}) {
+        if (!m) continue;
+        MB_REQUIRE(m->ld >= 1 && m->rpb >= 0 && m->bstride >= 0, "a row map needs ld >= 1, rpb >= 0 and bstride >= 0");
+        MB_REQUIRE(m->rpb == 0 || m->rpb <= M, "a row map's rows per batch exceed M");
+    }
+    MB_REQUIRE(A->rpb == 0 || M % A->rpb == 0, "A's rows per batch must divide M (whole batches are read)");
+    MB_REQUIRE(A->ld % 4 == 0 && (A->rpb == 0 || A->bstride % 4 == 0) && ldw % 4 == 0, "A and W row strides must be multiples of 4 floats");
+    MB_REQUIRE(ldw >= K, "W's row stride is shorter than K");
+    MB_REQUIRE(C->ld >= N && (!R || R->ld >= N), "an output or residual row stride is shorter than N");
+    MB_REQUIRE(reinterpret_cast<uintptr_t>(A->ptr) % 16 == 0 && reinterpret_cast<uintptr_t>(W) % 16 == 0, "A and W must be 16-byte aligned");
+    MB_REQUIRE(!gate || (gate_rpb >= 1 && gate_ld >= N), "a gate needs gate_rpb >= 1 and gate_ld >= N");
     GemmParams g{};
-    g.A = plain_map(A, lda); g.W = W; g.ldw = ldw; g.C = plain_map(C, ldc); g.bias = bias; g.act = act; g.alpha = alpha;
-    g.gate = gate; g.gate_ld = gate_ld; g.gate_rpb = gate_rpb > 0 ? gate_rpb : 1;
-    g.R = residual ? plain_map(residual, ldr) : RowMap{nullptr, 0, 0, 0};
-    g.M = M; g.N = N; g.K = K;
-    return launch_gemm(g, (cudaStream_t)stream, default_gemm_ctx());
-}
-
-extern "C" int mb200_op_gemm_tc(const float* A, int64_t lda, const float* W, int64_t ldw, float* C, int64_t ldc, const float* bias, int32_t act,
-                                float alpha, const float* residual, int64_t ldr, int32_t M, int32_t N, int32_t K, void* stream) {
-    GemmParams g{};
-    g.A = plain_map(A, lda); g.W = W; g.ldw = ldw; g.C = plain_map(C, ldc); g.bias = bias; g.act = act; g.alpha = alpha;
-    g.gate = nullptr; g.gate_ld = 0; g.gate_rpb = 1;
-    g.R = residual ? plain_map(residual, ldr) : RowMap{nullptr, 0, 0, 0};
+    g.A = batched_map(A->ptr, A->ld, A->rpb, A->bstride); g.W = W; g.ldw = ldw;
+    g.C = batched_map(C->ptr, C->ld, C->rpb, C->bstride); g.bias = bias; g.act = act; g.alpha = alpha;
+    g.gate = gate; g.gate_ld = gate ? gate_ld : 0; g.gate_rpb = gate ? gate_rpb : 1;
+    g.R = R ? batched_map(R->ptr, R->ld, R->rpb, R->bstride) : RowMap{nullptr, 0, 0, 0};
     g.M = M; g.N = N; g.K = K;
     GemmCtx* ctx = default_gemm_ctx();
-    int s = ctx->register_weight(W, (long long)N * ldw);
-    if (s) return s;
-    if (!tc_gemm_eligible(g, ctx)) {
-        ctx->unregister_weight(W);
-        MB_REQUIRE(false, "problem not eligible for the wgmma path (M >= 512, K % 4 == 0, 16-byte aligned operands)");
+    if (path == 2) {      // eligibility apart from the mirror, judged before anything is launched
+        const bool had = ctx->mirrors.count(W) != 0;
+        if (!had) ctx->mirrors[W] = Tf32Mirror{nullptr, nullptr};
+        const bool ok = tc_gemm_eligible(g, ctx);
+        if (!had) ctx->mirrors.erase(W);
+        MB_REQUIRE(ok, "problem not eligible for the wgmma path (tensor cores on, M >= 512, N >= 64, K >= 32, K % 4 == 0, A rows per batch a "
+                       "multiple of 128, 16-byte aligned operands and strides)");
     }
-    s = launch_gemm_tc(g, (cudaStream_t)stream, ctx);
-    cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (path != 1) OP_TRY(ctx->register_weight(W, (long long)(N - 1) * ldw + K));
+    int s = path == 2 ? launch_gemm_tc(g, st, ctx) : launch_gemm(g, st, ctx);
+    const cudaError_t e = cudaStreamSynchronize(st);
     ctx->unregister_weight(W);      // W belongs to the caller (a torch tensor whose address may be recycled)
     if (s) return s;
     MB_CUDA_CHECK(e);
@@ -86,24 +100,39 @@ extern "C" int mb200_op_gemm_tc(const float* A, int64_t lda, const float* W, int
 extern "C" int mb200_set_tensor_cores(int32_t enabled) { g_tc_enabled = enabled; return 0; }
 
 extern "C" int mb200_op_layernorm(const float* x, float* y, const float* w, const float* b, const float* shift, const float* scale,
-                                  int32_t rows_per_batch, int32_t rows, int32_t dim, float eps, void* stream) {
+                                  int64_t mod_ld, int32_t rows_per_batch, int32_t rows, int32_t dim, float eps, void* stream) {
+    MB_REQUIRE(x && y, "null argument");
+    MB_REQUIRE(!shift == !scale, "modulate needs both shift and scale");
+    MB_REQUIRE(!shift || mod_ld == 0 || mod_ld >= dim, "mod_ld is shorter than a row");
     LayerNormParams p{};
-    p.x = x; p.ldx = dim; p.y = y; p.ldy = dim; p.weight = w; p.bias = b; p.shift = shift; p.scale = scale; p.mod_ld = dim;
+    p.x = x; p.ldx = dim; p.y = y; p.ldy = dim; p.weight = w; p.bias = b; p.shift = shift; p.scale = scale; p.mod_ld = mod_ld > 0 ? mod_ld : dim;
     p.rows_per_batch = rows_per_batch > 0 ? rows_per_batch : 1; p.rows = rows; p.dim = dim; p.eps = eps;
     return launch_layernorm(p, (cudaStream_t)stream);
 }
 
-extern "C" int mb200_op_attention(const float* q, const float* k, const float* v, float* o, int32_t B, int32_t H, int32_t Tq, int32_t Tk,
-                                  float scale, int32_t mask_mode, int32_t q_pos0, const uint8_t* key_valid, int32_t band,
-                                  const uint8_t* dense_mask, void* stream) {
-    AttentionParams a{};
+extern "C" int mb200_op_attention(const float* q, int64_t q_ld, int64_t q_bs, const float* k, int64_t k_ld, int64_t k_bs, const float* v,
+                                  int64_t v_ld, int64_t v_bs, float* o, int64_t o_ld, int64_t o_bs, int32_t B, int32_t H, int32_t Tq, int32_t Tk,
+                                  float scale, int32_t mask_mode, int32_t q_pos0, const uint8_t* key_valid, int64_t key_valid_ld, int32_t band,
+                                  const uint8_t* dense_mask, const int32_t* kv_slot, void* stream) {
+    MB_REQUIRE(q && k && v && o, "null argument");
+    MB_REQUIRE(B >= 1 && H >= 1 && Tq >= 1 && Tk >= 1, "need B, H, Tq and Tk >= 1");
+    MB_REQUIRE(mask_mode >= MASK_NONE && mask_mode <= MASK_DENSE, "unknown mask mode");
+    MB_REQUIRE(mask_mode != MASK_DENSE || dense_mask, "a dense mask mode needs the mask");
+    MB_REQUIRE(!key_valid || key_valid_ld >= Tk, "key_valid_ld is shorter than Tk");
     const long long D = (long long)H * 64;
-    a.q = q; a.q_ld = D; a.q_bs = (long long)Tq * D;
-    a.k = k; a.k_ld = D; a.k_bs = (long long)Tk * D;
-    a.v = v; a.v_ld = D; a.v_bs = (long long)Tk * D;
-    a.o = o; a.o_ld = D; a.o_bs = (long long)Tq * D;
+    MB_REQUIRE(q_ld >= D && k_ld >= D && v_ld >= D && o_ld >= D, "a token stride is shorter than H * 64");
+    MB_REQUIRE(q_bs >= 0 && k_bs >= 0 && v_bs >= 0 && o_bs >= 0, "negative batch stride");
+    for (const void* ptr : {(const void*)q, (const void*)k, (const void*)v, (const void*)o})
+        MB_REQUIRE(reinterpret_cast<uintptr_t>(ptr) % 16 == 0, "q, k, v and o are read and written as float4: 16-byte alignment");
+    MB_REQUIRE(q_ld % 4 == 0 && k_ld % 4 == 0 && v_ld % 4 == 0 && o_ld % 4 == 0 && q_bs % 4 == 0 && k_bs % 4 == 0 && v_bs % 4 == 0 &&
+                   o_bs % 4 == 0, "attention strides must be multiples of 4");
+    AttentionParams a{};
+    a.q = q; a.q_ld = q_ld; a.q_bs = q_bs;
+    a.k = k; a.k_ld = k_ld; a.k_bs = k_bs;
+    a.v = v; a.v_ld = v_ld; a.v_bs = v_bs;
+    a.o = o; a.o_ld = o_ld; a.o_bs = o_bs;
     a.B = B; a.H = H; a.Tq = Tq; a.Tk = Tk; a.scale = scale; a.mask_mode = mask_mode; a.q_pos0 = q_pos0;
-    a.key_valid = key_valid; a.key_valid_ld = Tk; a.band = band; a.dense = dense_mask; a.kv_slot = nullptr;
+    a.key_valid = key_valid; a.key_valid_ld = key_valid_ld; a.band = band; a.dense = dense_mask; a.kv_slot = kv_slot;
     static AttnCtx op_ctx;                    // scratch of this kernel-level test entry point
     const int rc = launch_attention(a, (cudaStream_t)stream, &op_ctx);
     if (rc) return rc;
@@ -116,7 +145,6 @@ extern "C" int mb200_op_attention(const float* q, const float* k, const float* v
 
 // One decode-attention phase through launch_decode_attention / launch_decode_attention_ragged, with the scratch a token step gives them
 // (call state, split partials, tickets) owned here.
-#define OP_TRY(expr) do { int _s = (expr); if (_s) return _s; } while (0)
 namespace {
 struct OpScratch {
     void* p = nullptr; size_t bytes = 0;

@@ -25,49 +25,95 @@ def _f32c(t: torch.Tensor) -> torch.Tensor:
     return t
 
 
-def gemm(a, w, bias=None, act="none", alpha=1.0, residual=None, gate=None, gate_rows_per_batch=1):
-    """act(a @ w.T + bias) * alpha [* gate[row // rpb]] [+ residual]."""
+GEMM_PATHS = {"engine": 0, "simt": 1, "tc": 2}
+
+
+def _rowmap(t: torch.Tensor, what: str):
+    """RowMap of a float32 CUDA view: 2-D (rows, cols) -> rows at stride(0); 3-D (batches, rpb, cols) -> ld = stride(1), bstride =
+    stride(0), so `as_strided` views with overlapping rows and `expand`ed tables (stride(0) == 0) map directly.  Returns (map, rows)."""
+    assert t.is_cuda and t.dtype == torch.float32 and t.stride(-1) == 1, f"{what}: float32 CUDA view with unit column stride"
+    if t.dim() == 2:
+        return _lib.RowMapC(t.data_ptr(), t.stride(0), 0, 0), t.shape[0]
+    assert t.dim() == 3, f"{what}: 2-D (rows, cols) or 3-D (batches, rows per batch, cols)"
+    return _lib.RowMapC(t.data_ptr(), t.stride(1), t.shape[1], t.stride(0)), t.shape[0] * t.shape[1]
+
+
+def gemm_mapped(a, w, c, bias=None, act="none", alpha=1.0, residual=None, gate=None, gate_rows_per_batch=1, path="engine"):
+    """c = act(a @ w.T + bias) * alpha [* gate[row // gate_rows_per_batch]] [+ residual], written through the views' row maps
+    (`mb200_op_gemm_mapped`).  a (rows, K) or (batches, rpb, K); c and residual (rows, N) or (batches, rpb, N), the same row count
+    (residual may be c itself); w (N, K) and gate (groups, N) with unit column stride.  path "engine" dispatches as the engine does for a
+    registered weight, "simt" forces the fp32 kernel, "tc" the wgmma 3xTF32 kernel (an error if the problem is not eligible).  Returns c."""
     lib = _lib.load()
+    am, M = _rowmap(a, "a")
+    cm, Mc = _rowmap(c, "c")
+    assert w.is_cuda and w.dtype == torch.float32 and w.dim() == 2 and w.stride(1) == 1
+    N, K = w.shape
+    assert a.shape[-1] == K and c.shape[-1] == N and Mc == M, "shapes do not chain"
+    rm = None
+    if residual is not None:
+        rm, Mr = _rowmap(residual, "residual")
+        assert residual.shape[-1] == N and Mr == M
+    if gate is not None:
+        assert gate.is_cuda and gate.dtype == torch.float32 and gate.dim() == 2 and gate.stride(1) == 1 and gate.shape[1] == N
+    if bias is not None:
+        assert bias.is_cuda and bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == N
+    _lib.check(lib.mb200_op_gemm_mapped(am, _ptr(w), w.stride(0), cm, _ptr(bias), ACT[act], float(alpha), rm, _ptr(gate),
+                                        gate.stride(0) if gate is not None else 0, int(gate_rows_per_batch), M, N, K, GEMM_PATHS[path],
+                                        _stream()))
+    return c
+
+
+def gemm(a, w, bias=None, act="none", alpha=1.0, residual=None, gate=None, gate_rows_per_batch=1):
+    """act(a @ w.T + bias) * alpha [* gate[row // rpb]] [+ residual], on the fp32 SIMT kernel."""
     a, w = _f32c(a), _f32c(w)
-    M, K = a.shape
-    N = w.shape[0]
-    out = torch.empty(M, N, device=a.device, dtype=torch.float32)
-    _lib.check(lib.mb200_op_gemm(_ptr(a), K, _ptr(w), K, _ptr(out), N, _ptr(bias), ACT[act], float(alpha), _ptr(residual), N,
-                                 _ptr(gate), (gate.shape[1] if gate is not None else 0), int(gate_rows_per_batch), M, N, K, _stream()))
-    return out
+    out = torch.empty(a.shape[0], w.shape[0], device=a.device, dtype=torch.float32)
+    return gemm_mapped(a, w, out, bias, act, alpha, residual, gate, gate_rows_per_batch, path="simt")
 
 
 def gemm_tc(a, w, bias=None, act="none", alpha=1.0, residual=None):
     """Same contract as `gemm`, forced through the wgmma 3xTF32 kernel."""
-    lib = _lib.load()
     a, w = _f32c(a), _f32c(w)
-    M, K = a.shape
-    N = w.shape[0]
-    out = torch.empty(M, N, device=a.device, dtype=torch.float32)
-    _lib.check(lib.mb200_op_gemm_tc(_ptr(a), K, _ptr(w), K, _ptr(out), N, _ptr(bias), ACT[act], float(alpha), _ptr(residual), N, M, N, K, _stream()))
-    return out
+    out = torch.empty(a.shape[0], w.shape[0], device=a.device, dtype=torch.float32)
+    return gemm_mapped(a, w, out, bias, act, alpha, residual, path="tc")
 
 
 def layernorm(x, weight=None, bias=None, shift=None, scale=None, rows_per_batch=1, eps=1e-5):
+    """LayerNorm of the rows of x: affine (weight / bias), or modulate by shift / scale (batches, dim) rows, which may be views into a
+    wider buffer (their common row stride is the modulation stride)."""
     lib = _lib.load()
     x = _f32c(x)
     rows, dim = x.shape
     y = torch.empty_like(x)
-    _lib.check(lib.mb200_op_layernorm(_ptr(x), _ptr(y), _ptr(weight), _ptr(bias), _ptr(shift), _ptr(scale), int(rows_per_batch), rows, dim,
-                                      float(eps), _stream()))
+    mod_ld = 0
+    if shift is not None:
+        assert shift.stride() == scale.stride() and shift.stride(1) == 1, "shift and scale rows at one stride"
+        mod_ld = shift.stride(0)
+    _lib.check(lib.mb200_op_layernorm(_ptr(x), _ptr(y), _ptr(weight), _ptr(bias), _ptr(shift), _ptr(scale), mod_ld, int(rows_per_batch), rows,
+                                      dim, float(eps), _stream()))
     return y
 
 
-def attention(q, k, v, heads, scale=1.0, mask="none", q_pos0=0, key_valid=None, band=0, dense_mask=None):
-    """q (B, Tq, H*64), k/v (B, Tk, H*64) token-major -> (B, Tq, H*64)."""
+def attention(q, k, v, heads, scale=1.0, mask="none", q_pos0=0, key_valid=None, band=0, dense_mask=None, kv_slot=None, out=None):
+    """q (B, Tq, >= H*64), k / v (B or slots, Tk, >= H*64) token-major views with unit column stride (column slices of one qkv buffer,
+    the K | V cache) -> out (B, Tq, H*64), allocated when not given.  key_valid (B, >= Tk) uint8 view; kv_slot int32 (B,): batch row b
+    reads K / V of batch index kv_slot[b]."""
     lib = _lib.load()
-    q, k, v = _f32c(q), _f32c(k), _f32c(v)
+    for t in (q, k, v):
+        assert t.is_cuda and t.dtype == torch.float32 and t.dim() == 3 and t.stride(2) == 1
     B, Tq, _ = q.shape
     Tk = k.shape[1]
-    o = torch.empty_like(q)
-    _lib.check(lib.mb200_op_attention(_ptr(q), _ptr(k), _ptr(v), _ptr(o), B, heads, Tq, Tk, float(scale), MASK[mask], int(q_pos0),
-                                      _ptr(key_valid), int(band), _ptr(dense_mask), _stream()))
-    return o
+    if out is None:
+        out = torch.empty(B, Tq, heads * 64, device=q.device, dtype=torch.float32)
+    assert out.is_cuda and out.dtype == torch.float32 and out.dim() == 3 and out.stride(2) == 1
+    if key_valid is not None:
+        assert key_valid.is_cuda and key_valid.dtype == torch.uint8 and key_valid.stride(1) == 1
+    if kv_slot is not None:
+        assert kv_slot.is_cuda and kv_slot.dtype == torch.int32 and kv_slot.is_contiguous() and kv_slot.numel() == B
+    _lib.check(lib.mb200_op_attention(_ptr(q), q.stride(1), q.stride(0), _ptr(k), k.stride(1), k.stride(0), _ptr(v), v.stride(1), v.stride(0),
+                                      _ptr(out), out.stride(1), out.stride(0), B, heads, Tq, Tk, float(scale), MASK[mask], int(q_pos0),
+                                      _ptr(key_valid), key_valid.stride(0) if key_valid is not None else 0, int(band), _ptr(dense_mask),
+                                      _ptr(kv_slot), _stream()))
+    return out
 
 
 DECODE_ATTENTION_FORMS = {"default": 0, "cta128": 1, "cta64": 2, "warp": 3}
